@@ -64,11 +64,32 @@ def parse():
     ap.add_argument("--train", type=int, default=0, help="data-parallel training step instead of independent views")
     ap.add_argument("--views-per-step", type=int, default=2, help="--train: views per rank per optimizer step")
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed (render outputs, normal map, "
+                         "parameter gradients) as DIR/<name>.npy in float32; an array of more than 2^20 elements is "
+                         "flattened and reduced to a fixed, seeded sample of 2^20 of them (the same positions in every run)")
+    a = ap.parse_args()
+    if a.dump_outputs and (a.train or a.impl != "new"):
+        ap.error("--dump-outputs applies to the independent-view benchmark of this framework (--train 0 --impl new)")
+    return a
+
+
+DUMP_MAX = 1 << 20  # elements per dumped array: at most 4 MB each, 11 arrays in all
+
+
+def dump_outputs(path, arrays):
+    """arrays: {name: tensor}.  Deterministic: the sample of a large array depends on its size only."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    for name, t in arrays.items():
+        x = t.detach().float().cpu().numpy().reshape(-1) if t.dtype != torch.float64 else t.detach().cpu().numpy().reshape(-1)
+        if x.size > DUMP_MAX:
+            x = x[np.sort(np.random.RandomState(0).choice(x.size, DUMP_MAX, replace=False))]
+        np.save(os.path.join(path, name + ".npy"), x if x.size != t.numel() else x.reshape(tuple(t.shape)))
 
 
 class ClockSampler:
-    """SM clock / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe) through NVML: a
+    """SM clock / throttle reasons sampled DURING the timed region through NVML: a
     background thread every `period` seconds plus one sample when the host has enqueued the last step (the GPU is
     still executing the region then).  NVML is opened before the region.  (Polling `nvidia-smi -lms` from a child
     process stalled the CUDA launch path by several ms per step on these hosts; sparse NVML calls do not.)"""
@@ -362,7 +383,7 @@ def run_reference(a):
         "gpu_launches": 0,
         "cpu_baseline": {"value": v, "unit": "views/s", "cores": 1, "kind": "reference",
                          "sample": "the reference has no CPU implementation of this path: its own CUDA extension "
-                                   "(unmodified sources compiled for sm_100a) driven by one host thread"},
+                                   "(unmodified sources compiled for sm_90a) driven by one host thread"},
     }
     out["native_so_loaded"] = mapped_repo_libraries()
     assert not any("libgsr_b200" in x for x in out["native_so_loaded"]), "the reference arm must not map libgsr_b200.so"
@@ -393,11 +414,14 @@ def run_new(a):
     def normal(cam, depth):
         return ops.depth2normal(depth, cam.fx, cam.fy, cam.cx, cam.cy)
 
+    last = {}  # outputs of the latest eager step (--dump-outputs)
+
     def step(cam, rend=renderer):
         if not backward:
             with torch.no_grad():
                 out = rend.render(cam, model)
                 n = normal(cam, out["rendered_depth"][0])
+            last.update(out=out, normal=n)
             return out["rendered_depth"].mean() + 0.0 * n[0, 0, 0]
         for p in params:
             p.grad = None
@@ -405,6 +429,7 @@ def run_new(a):
         loss = loss_fn(out)
         loss.backward()
         n = normal(cam, out["rendered_depth"].detach()[0])
+        last.update(out=out, normal=n)
         return loss.detach() + 0.0 * n[0, 0, 0]
 
     def sync_all():
@@ -494,6 +519,16 @@ def run_new(a):
     clocks = sampler.stop()
     assert bool(torch.isfinite(all_losses).all())
     _C.check_pipeline(wait=True)
+    if a.dump_outputs and rank == 0:
+        if graphed is not None:
+            gs = graphed[(K - 1) % nstreams]
+            out, n, grads = (gs.out, gs.extra, gs.grads) if backward else (gs.loss, gs.extra, [])
+        else:
+            out, n, grads = last["out"], last["normal"], ([p.grad for p in params] if backward else [])
+        arrays = {k: out[k] for k in ("render", "rendered_depth", "rendered_median_depth", "rendered_final_opacity")}
+        arrays["normal"] = n
+        arrays.update({"grad_" + name: g for name, g in zip(("xyz", "scale", "rot", "opacity", "f_dc", "f_rest"), grads)})
+        dump_outputs(a.dump_outputs, arrays)
 
     # ---------------- leg 1b: per-kernel CUDA-event times over the same K steps (library-side events around every
     # launch on the caller's stream; eager launches, one stream).  Kept out of leg 1. ----------------
@@ -561,8 +596,8 @@ def run_new(a):
     pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pk):
         peaks = json.load(open(pk))
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s (not measured)"
     _C.set_pipelined(False)
     stats = []
     e = torch.Tensor([])
@@ -580,10 +615,6 @@ def run_new(a):
     if backward:
         grp_ms.update(render_bwd=stage_ms["render_bwd"], preprocess_bwd=stage_ms["preprocess_bwd"])
     stages_out = {}
-    traffic = {}
-    tf = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tf):
-        traffic = json.load(open(tf))
     for k in grp_ms:
         gbs = ab[k] / (grp_ms[k] * 1e-3) / 1e9 if grp_ms[k] > 0 else 0.0
         stages_out[k] = {"ms": round(grp_ms[k], 4), "algorithmic_MB": round(ab[k] / 1e6, 2), "GBps": round(gbs, 1),
@@ -591,14 +622,11 @@ def run_new(a):
     dom = max(grp_ms, key=lambda k: grp_ms[k])
     roof = {"kernel": dom, "bound": "hbm", "achieved": stages_out[dom]["GBps"], "peak": hbm_peak, "unit": "GB/s",
             "frac": stages_out[dom]["frac"],
-            "traffic": traffic.get(dom) if a.config in ("cfg3", "cfg4") else None,
-            "traffic_source": "constant from the committed ncu --set full capture (profiles/ncu_traffic.json), not "
-                              "measured in this run",
+            "traffic": None,
+            "traffic_source": "not measured (no Nsight Compute capture)",
             "peak_source": peak_src,
-            "issue_active_pct": (traffic.get("_issue_active_pct") or {}).get(dom),
-            "note": "FP32/SFU-bound compositing: HBM fraction is low by construction (DESIGN.md, Roofline honesty); "
-                    "issue_active_pct = smsp__issue_active of this kernel in the committed ncu capture (a constant like "
-                    "`traffic`): the resource it is actually bound by"}
+            "issue_active_pct": None,
+            "note": "FP32/SFU-bound compositing: HBM fraction is low by construction (DESIGN.md, Roofline honesty)"}
     stages_out["_kernels_ms"] = {k: round(v, 4) for k, v in stage_ms.items()}
     stages_out["_workload"] = {"R": R, "R_binned": R_binned, "R_need": R_need, "P_visible": P_vis,
                                "tile_instances_first_view": stats[0][4],
@@ -616,7 +644,7 @@ def run_new(a):
                    "streams_per_gpu": nstreams,
                    "launch": ("one CUDA graph per view, fixed binning capacity "
                               f"{graphed[0].capacity}" if graphed is not None else "eager kernel launches"),
-                   "l2": "inputs larger than L2 (Gaussian parameters + per-view outputs vs 126 MB)",
+                   "l2": "inputs larger than L2 (Gaussian parameters + per-view outputs vs 50 MB)",
                    "activations": ("fused into the projection kernel (fused_activations=True)" if a.fused else
                                    "torch ops per view (reference op sequence)"),
                    "forward_mode": "pipelined (no host sync; overflow-checked)" if a.pipelined else

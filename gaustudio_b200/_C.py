@@ -187,7 +187,7 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")  # rasterize_points.cu:57-59
     if not means3D.is_cuda:
-        raise RuntimeError("gaustudio_b200 runs on CUDA (sm_100a) only; means3D must be a CUDA tensor")
+        raise RuntimeError("gaustudio_b200 runs on CUDA (sm_90a) only; means3D must be a CUDA tensor")
     L = _lib.lib()
     dev = means3D.device
     P, H, W = means3D.size(0), int(image_height), int(image_width)

@@ -1,4 +1,4 @@
-"""Builds libgsr_b200.so (hand-written sm_100a CUDA + the C ABI of include/gsr.h) in-tree with nvcc.
+"""Builds libgsr_b200.so (hand-written sm_90a (H100) CUDA + the C ABI of include/gsr.h) in-tree with nvcc.
 
 No fast-math: the reference extension is built without it ($RAST/setup.py:29), and the per-pair
 thresholds of the compositing loop need the same precise expf / IEEE division.
@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 SOURCES = ["gsr_api.cu", "gsr_preprocess.cu", "gsr_binning.cu", "gsr_render.cu", "gsr_extract.cu"]
 LIB = os.path.join(HERE, "libgsr_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
          "--extended-lambda", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 
 

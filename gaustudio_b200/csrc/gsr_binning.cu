@@ -140,12 +140,11 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_tile_scan(ImageView im, int T,
 #if GSR_WITH_CLUSTER_SCAN
 // ---- level 1a, cluster form: the same scan by a thread-block cluster of 8 CTAs -- EXPERIMENTAL, not in the default build
 // Compiled only with -DGSR_WITH_CLUSTER_SCAN=1 (tools/build_variants.py cluster_scan) and then selected at run time with
-// GSR_SCAN_CLUSTER=1.  It is 2.5x faster than the single-CTA scan (0.015 vs 0.037 ms at 1080p) and passed the whole GPU
-// suite, but with it the first un-fused render of tests/test_gpu_api.py::test_fused_path_with_mostly_culled_ctas_...
-// came out slightly different (a few 1e-3 on ~140 of 180 tiles, not reproducible on re-render) in 4 of 33 fresh-process
-// runs, against 0 of 29 with the single-CTA scan (profiles/r2c_flake_arms.md); the cause was not found in the GPU time
-// that was left, so the validated single-CTA kernel stays the product path (DESIGN.md 3.5).
-// The single-CTA scan is pure latency on one SM (37 us at 1080p: 8160 tiles x 16 counters through one SM's load path,
+// GSR_SCAN_CLUSTER=1.  It is faster than the single-CTA scan and passed the whole GPU suite, but with it the first
+// un-fused render of tests/test_gpu_api.py::test_fused_path_with_mostly_culled_ctas_... came out slightly different
+// (not reproducible on re-render) more often than without it; the cause was not found, so the validated single-CTA
+// kernel stays the product path (DESIGN.md 3.5).
+// The single-CTA scan is pure latency on one SM (at 1080p: 8160 tiles x 16 counters through one SM's load path,
 // twice, plus a counting sort with contended shared-memory atomics).  Here every thread owns ONE tile per round (a round
 // = 8 x 1024 tiles: a 1080p image is one round), its 16 counters stay in registers between the total and the cursor
 // pass, the 8 CTAs exchange their round totals through distributed shared memory (one cluster barrier per round), and

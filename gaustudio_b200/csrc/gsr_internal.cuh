@@ -1,5 +1,5 @@
 // Internal declarations of libgsr_b200: buffer layouts, launch wrappers, device helpers.
-// B200 (sm_100a) only.  Not part of the public ABI (that is include/gsr.h).
+// H100 (sm_90a) only.  Not part of the public ABI (that is include/gsr.h).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -121,9 +121,8 @@ void launch_tile_scan(ImageView im, int T, cudaStream_t st);
 int set_tile_order(int mode);  // gsr_set_tile_order
 void launch_scatter(int P, int gx, int T, GeomView g, ImageView im, BinView b, cudaStream_t st);
 void launch_tile_sort(int T, GeomView g, ImageView im, BinView b, cudaStream_t st);
-// splat_tensor_map: a CUtensorMap over the [P][12 float] splat array (TMA gather4 staging) or nullptr (LDGSTS staging)
-void launch_render_fwd(int W, int H, int gx, int gy, ImageView im, BinView b, GeomView g, const void* splat_tensor_map,
-                       float* out_color, float* out_depth, float* out_median, float* out_opacity, cudaStream_t st);
+// tma: stage the record batches with TMA bulk copies instead of LDGSTS (GSR_FWD_TMA=1)
+void launch_render_fwd(int W, int H, int gx, int gy, ImageView im, BinView b, GeomView g, bool tma, float* out_color, float* out_depth, float* out_median, float* out_opacity, cudaStream_t st);
 void launch_render_bwd(int W, int H, int gx, int gy, const float* bg, ImageView im, BinView b, GeomView g,
                        const float* dL_dpix, const float* dL_ddepth, const float* dL_dmedian,
                        const float* dL_dopacity, cudaStream_t st);

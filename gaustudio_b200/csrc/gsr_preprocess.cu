@@ -5,7 +5,7 @@
 //   forward : $RAST/cuda_rasterizer/forward.cu:20-71 (SH), 74-113 (cov2D), 118-152 (cov3D), 155-256 (K1)
 //   backward: $RAST/cuda_rasterizer/backward.cu:144-274 (K6), 346-412 (K7), 20-139 (SH), 278-341 (cov3D)
 //   helpers : $RAST/cuda_rasterizer/auxiliary.h:41-77,107-117,139-164
-// Design differences (B200): one packed 48-B splat record per Gaussian instead of five SoA arrays; per-tile
+// Design differences (H100): one packed 48-B splat record per Gaussian instead of five SoA arrays; per-tile
 // instance counts are accumulated here (no per-Gaussian prefix scan, no duplicateWithKeys offsets); K6 and
 // K7 are one kernel and write every output element (no torch::zeros pre-pass, rasterize_points.cu:160-169).
 #include "gsr_internal.cuh"
@@ -31,8 +31,8 @@ struct V3 { float x, y, z; };
 // PRE_THREADS x 12 B of f_dc land in shared memory while the threads do the projection math; rows of 3 / 45 words have
 // odd strides, so per-thread row reads are bank-conflict free.  The backward writes its SH gradients into the
 // same rows and ships the block with one bulk store per tensor.
-// CTA size of the projection kernels: 128 measured best with several views in flight (64 / 128 / 256 in
-// profiles/r2_ab_block_sizes.json): smaller CTAs slot into the SMs as the compositing CTAs of other streams retire
+// CTA size of the projection kernels: 128 measured best of 64 / 128 / 256 with several views in flight (A/B not
+// repeated on the H100): smaller CTAs slot into the SMs as the compositing CTAs of other streams retire
 #ifndef GSR_PRE_THREADS
 #define GSR_PRE_THREADS 128
 #endif
@@ -320,7 +320,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 1024 / PRE_THREADS) k_preprocess_
           unsigned char cl = 0;
           if (a.colors_precomp == nullptr) {
             // computeColorFromSH, forward.cu:20-71 (coefficient stride M, degree D: quirk 13).  Written with
-            // explicit mul / fma intrinsics in the contraction the reference's sm_100a SASS ends up with (ptxas
+            // explicit mul / fma intrinsics in the contraction the reference's sm_90a SASS ends up with (ptxas
             // fuses its mul+add/sub pairs): weight_k rounded on its own, then res = fma(weight_k, sh_k, res).
             // coefficient 0 and coefficients >= 1 may live in two tensors (fused path: f_dc / f_rest)
             const float* sh0 = a.fused ? a.f_dc + (size_t)idx * 3 : a.shs + (size_t)idx * a.M * 3;

@@ -6,7 +6,7 @@
 // precise expf), thresholds (power>0, alpha<1/255, T<1e-4, median at T crossing 0.5), contributor counting
 // and un-normalised depth / no-background colour outputs.
 //
-// What is different (B200):
+// What is different (H100):
 //  * a dedicated producer warp walks the tile's sorted index list and stages the 48-byte splat records of
 //    the next batches into a shared-memory ring with asynchronous 16-byte copies (cp.async, completion on an
 //    mbarrier), NSTAGE batches ahead of the consumer warps -- no CTA-wide barrier in the loop, and
@@ -31,7 +31,6 @@
 #include "gsr_internal.cuh"
 #include <cstdlib>
 #include <cstring>
-#include <cuda.h>  // CUtensorMap (type only; the encoder is resolved at run time in gsr_api.cu)
 
 namespace gsr {
 
@@ -80,39 +79,26 @@ __device__ __forceinline__ void stage_gather(float4* dst, const float4* __restri
   }
   cp_async_arrive(full);
 }
-// ---- TMA tile::gather4 staging (opt-in, GSR_FWD_TMA=1; DESIGN.md 3.2) -----------------------------------------
-// One instruction fetches FOUR 48-byte records, given their row indices in the [P][12 float] splat array, into
-// 192 contiguous bytes of shared memory.  The destination of a tensor copy must be 128-byte aligned, so the staged
-// batch is laid out in 256-byte groups of four records (192 B used): record r sits at (r / 4) * 256 + (r % 4) * 48.
-constexpr int TMA_GROUP_F4 = 16;                                   // float4 per group of four records
-constexpr int TMA_STAGE_F4 = (RB / 4) * TMA_GROUP_F4;              // 8 KB per stage
-__device__ __forceinline__ void tma_gather4(void* dst_smem, const CUtensorMap* tm, int r0, int r1, int r2, int r3,
-                                            unsigned long long* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile::gather4.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-      "%6, %7}], [%2];" ::"r"(smem_u32(dst_smem)),
-      "l"(tm), "r"(smem_u32(bar)), "r"(0), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
-      : "memory");
+// ---- TMA bulk-copy staging (opt-in, GSR_FWD_TMA=1; DESIGN.md 3.2) ---------------------------------------------
+// One cp.async.bulk per record: the TMA engine copies the 48 contiguous bytes of splat[id] into the stage (both ends
+// 16-byte aligned), and the copy completes its bytes on the stage's `full` barrier.  Same stage layout as the
+// LDGSTS flavour.
+__device__ __forceinline__ void tma_copy(void* dst_smem, const void* src_gmem, unsigned bytes, unsigned long long* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                   smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
 }
 __device__ __forceinline__ void mbar_arrive_expect(unsigned long long* bar, unsigned bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-// producer warp, TMA flavour: lane l fetches records 4l .. 4l+3 of the batch with one gather4 (indices past the end of
-// the batch repeat the last valid one: the slots are never read)
-__device__ __forceinline__ void stage_gather_tma(float4* dst, const CUtensorMap* tm, const uint32_t* __restrict__ ids,
-                                                 int cnt, int lane, unsigned long long* full) {
-  const int r = 4 * lane;
-  if (r < cnt) {
-    const int last = cnt - 1;
-    const int i0 = (int)ids[r], i1 = (int)ids[min(r + 1, last)], i2 = (int)ids[min(r + 2, last)], i3 = (int)ids[min(r + 3, last)];
-    mbar_arrive_expect(full, 4 * SPLAT_BYTES);
-    tma_gather4(dst + lane * TMA_GROUP_F4, tm, i0, i1, i2, i3, full);
-  } else {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(full)) : "memory");
-  }
-}
-template <bool TMA> __device__ __forceinline__ const float4* rec_at(const float4* sb, int j) {
-  return TMA ? sb + (j >> 2) * TMA_GROUP_F4 + (j & 3) * SPLAT_F4 : sb + j * SPLAT_F4;
+// producer warp, TMA flavour: lane l copies records l, l+32, ...; each lane first announces its bytes with its one
+// arrival on `full` (initialised for 32), so the phase completes once all 32 lanes arrived and every byte landed
+__device__ __forceinline__ void stage_gather_tma(float4* dst, const float4* __restrict__ splat,
+                                                 const uint32_t* __restrict__ ids, int cnt, int lane,
+                                                 unsigned long long* full) {
+  const int mine = cnt > lane ? (cnt - lane + 31) / 32 : 0;
+  mbar_arrive_expect(full, (unsigned)(mine * SPLAT_BYTES));
+  for (int r = lane; r < cnt; r += 32) tma_copy(dst + r * SPLAT_F4, splat + (size_t)ids[r] * SPLAT_F4, SPLAT_BYTES, full);
 }
 
 __device__ __forceinline__ void mbar_arrive(unsigned long long* bar) {
@@ -192,12 +178,11 @@ constexpr int FWD_THREADS = TILE_PIX + 32;
 template <bool TMA>
 __global__ void __launch_bounds__(FWD_THREADS) k_render_fwd(int W, int H, int gx, ImageView im, BinView bin,
                                                             const float4* __restrict__ splat,
-                                                            const __grid_constant__ CUtensorMap tmap,
                                                             float* __restrict__ out_color,
                                                             float* __restrict__ out_depth,
                                                             float* __restrict__ out_median,
                                                             float* __restrict__ out_opacity) {
-  __shared__ __align__(128) RingT<TMA ? TMA_STAGE_F4 : STAGE_F4> ring;
+  __shared__ __align__(128) Ring ring;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int tile = (int)im.tile_order[blockIdx.x], tx = tile % gx, ty = tile / gx;  // longest tiles first
   const uint2 range = im.tile_range[tile];
@@ -218,7 +203,7 @@ __global__ void __launch_bounds__(FWD_THREADS) k_render_fwd(int W, int H, int gx
         stop = *(volatile unsigned*)&ring.ndone == NBLK;  // every pixel of the tile is finished
       }
       if (__shfl_sync(FULL, stop, 0)) break;
-      if (TMA) stage_gather_tma(ring.buf[s], &tmap, ids + b * RB, min(RB, n - b * RB), lane, &ring.full[s]);
+      if (TMA) stage_gather_tma(ring.buf[s], splat, ids + b * RB, min(RB, n - b * RB), lane, &ring.full[s]);
       else stage_gather(ring.buf[s], splat, ids + b * RB, min(RB, n - b * RB), lane, &ring.full[s]);
       issued = b + 1;
     }
@@ -265,7 +250,7 @@ __global__ void __launch_bounds__(FWD_THREADS) k_render_fwd(int W, int H, int gx
       const int j = base + lane;
       bool keep = false;
       if (j < cnt) {
-        const float4* cr = rec_at<TMA>(sb, j);
+        const float4* cr = sb + j * SPLAT_F4;
         keep = may_touch(cull_prep(cr[0], cr[1], cr[2].w), rx0, ry0, rx1, ry1);
       }
       unsigned mask = __ballot_sync(FULL, keep);
@@ -273,7 +258,7 @@ __global__ void __launch_bounds__(FWD_THREADS) k_render_fwd(int W, int H, int gx
       while (mask) {
         const int bit = __ffs(mask) - 1;
         mask &= mask - 1;
-        const float4* rec = rec_at<TMA>(sb, base + bit);
+        const float4* rec = sb + (base + bit) * SPLAT_F4;
         const float4 q0 = rec[0], q1 = rec[1];
         // forward.cu:343-356 with the contraction of the reference SASS (SURVEY.md A.4)
         const float dx = q0.x - pxf, dy = q0.y - pyf;
@@ -348,7 +333,7 @@ template <int NSUB> __device__ __forceinline__ int blk_ky(int w, int s) {
 #ifndef GSR_BWD_BOUND_EXTRA
 #define GSR_BWD_BOUND_EXTRA 0
 #endif
-// 1 (default): the compositing backward evaluates exp with one ex2.approx; 0: precise expf (A/B: profiles/r2_ab_bwd_loop.json)
+// 1 (default): the compositing backward evaluates exp with one ex2.approx; 0: precise expf (chosen by A/B)
 #ifndef GSR_BWD_FASTEXP
 #define GSR_BWD_FASTEXP 1
 #endif
@@ -559,25 +544,16 @@ template <typename K> static void allow_pad(K kernel) {
   if (render_pad()) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)render_pad());
 }
 
-void launch_render_fwd(int W, int H, int gx, int gy, ImageView im, BinView b, GeomView g, const void* splat_tensor_map,
-                       float* out_color, float* out_depth, float* out_median, float* out_opacity, cudaStream_t st) {
-  if (splat_tensor_map) {
-    allow_pad(k_render_fwd<true>);
-    k_render_fwd<true><<<gx * gy, FWD_THREADS, render_pad(), st>>>(W, H, gx, im, b, g.splat,
-                                                        *static_cast<const CUtensorMap*>(splat_tensor_map), out_color,
-                                                        out_depth, out_median, out_opacity);
-  } else {
-    CUtensorMap none;
-    memset(&none, 0, sizeof(none));
-    allow_pad(k_render_fwd<false>);
-    k_render_fwd<false><<<gx * gy, FWD_THREADS, render_pad(), st>>>(W, H, gx, im, b, g.splat, none, out_color, out_depth, out_median,
-                                                         out_opacity);
-  }
+void launch_render_fwd(int W, int H, int gx, int gy, ImageView im, BinView b, GeomView g, bool tma, float* out_color,
+                       float* out_depth, float* out_median, float* out_opacity, cudaStream_t st) {
+  auto kernel = tma ? k_render_fwd<true> : k_render_fwd<false>;
+  allow_pad(kernel);
+  kernel<<<gx * gy, FWD_THREADS, render_pad(), st>>>(W, H, gx, im, b, g.splat, out_color, out_depth, out_median, out_opacity);
 }
 
 // Pixels per lane of the compositing backward: 1 (default) or 2 (GSR_BWD_NSUB=2, read once per process).  The A/B on
-// cfg 3 (profiles/r2_ab_bwd_variants.json: 1, 2, 4 and 8 pixels per lane, two occupancy targets each) has one pixel
-// per lane fastest -- fewer reductions per Gaussian do not make up for the resident warps the extra registers cost --
+// cfg 3 (1, 2, 4 and 8 pixels per lane, two occupancy targets each; not repeated on the H100) had one pixel per lane
+// fastest -- fewer reductions per Gaussian do not make up for the resident warps the extra registers cost --
 // so only the two-pixel variant is kept as a validated alternative (tests/test_gpu_ring_stress.py).
 static int bwd_nsub() {
   static const int v = [] { const char* e = getenv("GSR_BWD_NSUB"); return (e && e[0] == '2') ? 2 : 1; }();

@@ -41,7 +41,7 @@ class VanillaRenderer(BaseRenderer):
         'convert_SHs_python': False,
         'compute_cov3D_python': False,
         'debug': False,
-        # B200 extension (off by default = the reference's op sequence): apply exp / sigmoid / normalize /
+        # H100 extension (off by default = the reference's op sequence): apply exp / sigmoid / normalize /
         # cat(f_dc, f_rest) inside the projection kernel instead of as per-view torch ops (SURVEY.md §8f rank 1)
         'fused_activations': False,
     }

@@ -1,4 +1,4 @@
-/* gsr.h -- C ABI of the B200-native differentiable 3DGS tile rasterizer (libgsr_b200.so).
+/* gsr.h -- C ABI of the H100-native differentiable 3DGS tile rasterizer (libgsr_b200.so).
  *
  * This is the drop-in seam for the torch-free core of the reference rasterizer,
  *   CudaRasterizer::Rasterizer::{forward, backward, markVisible}

@@ -1,12 +1,14 @@
 """-m gpu: the reference's own pybind surface (`rasterize_gaussians`, `rasterize_gaussians_backward`, `mark_visible`;
 ext.cpp:15-19) rebuilt on top of the C ABI -- integration/rasterize_points_gsr.cpp, the file INTEGRATION.md section 3
-hands a maintainer -- must give the same results as the unmodified reference extension when both are driven by the
-same autograd wrapper (oracle/ref_driver.RefRasterize: the argument packing of the reference's Python package)."""
+hands a maintainer -- must give the same results as the unmodified reference extension (golden data, tests/refgold.py)
+when driven by the same autograd wrapper (oracle/ref_driver.RefRasterize: the argument packing of the reference's
+Python package)."""
 import numpy as np
 import pytest
 import torch
 
 import gpu_util as U
+import refgold
 import scenes
 from integration import build_binding
 from oracle import ref_driver
@@ -24,22 +26,22 @@ def binding():
 
 @pytest.mark.parametrize("case", "ABCD")
 def test_binding_matches_reference_extension(binding, case):
-    if not ref_driver.available():
-        pytest.skip("oracle/_ref/_refC.so not present")
     s = scenes.scene(case)
     dev = torch.device("cuda")
     # forward AND backward of the run must go through `binding`: keep it selected for the whole run_torch call
-    ref_mod = ref_driver.module()
+    ref_mod = ref_driver._mod
     ref_driver._mod = binding
     try:
         new = scenes.run_torch(s, ref_driver.rasterize, dev)
     finally:
         ref_driver._mod = ref_mod
-    ref = scenes.run_torch(s, ref_driver.rasterize, dev)
+    ref = refgold.reference(f"case_{case}", lambda: scenes.run_torch(s, U.ref_rasterize, dev))
     for k in ("color", "depth", "median", "opacity", "radii"):
-        assert np.array_equal(new[k], ref[k]), k
-    for k in sorted(k for k in ref if k.startswith("g_")):
-        U.assert_grads_close(new[k], ref[k], what=f"{case}:{k}")
+        ref.assert_equal(k, new[k])
+    assert sorted(k for k in new if k.startswith("g_")) == sorted(k for k in ref.names() if k.startswith("g_"))
+    for k in sorted(k for k in new if k.startswith("g_")):
+        a, b, scale = ref.pair(k, new[k])
+        U.assert_grads_close(a, b, scale=scale, what=f"{case}:{k}")
 
 
 def test_binding_mark_visible_and_empty_input(binding):

@@ -1,7 +1,7 @@
 """-m gpu parity tests: the CUDA path (through the reference-shaped Python API -> ctypes -> C ABI) against
- (1) the UNMODIFIED reference extension compiled for sm_100a (oracle/_ref), on the same device,
- (2) the committed golden fixtures that extension produced on a B200 (tests/golden/ref_case_*.npz),
- (3) the CPU oracle.
+ (1) what the UNMODIFIED reference extension (oracle/_ref) computed on the same inputs on an H100, stored under
+     tests/golden (tests/refgold.py: refgold_*.npz; ref_case_*.npz with the reference's sorted lists),
+ (2) the CPU oracle.
 Tolerances: BASELINE.json -- 1e-4 max-abs on images, 1e-3 relative on gradients.  Against the reference on the
 same GPU the forward is expected to be BIT-EXACT (same arithmetic, same order), which is asserted."""
 import os
@@ -11,6 +11,7 @@ import pytest
 import torch
 
 import gpu_util as U
+import refgold
 import scenes
 from oracle import ref_driver
 
@@ -25,17 +26,16 @@ def _grad_keys(r):
 
 @pytest.mark.parametrize("case", "ABCD")
 def test_matches_compiled_reference(case):
-    if not ref_driver.available():
-        pytest.skip("oracle/_ref/_refC.so not present")
     s = scenes.scene(case)
     dev = torch.device("cuda")
     new = scenes.run_torch(s, U.new_rasterize, dev)
-    ref = scenes.run_torch(s, U.ref_rasterize, dev)
+    ref = refgold.reference(f"case_{case}", lambda: scenes.run_torch(s, U.ref_rasterize, dev))
     for k in FWD + ("radii",):
-        assert np.array_equal(new[k], ref[k]), f"{k} not bit-identical to the reference"
-    assert _grad_keys(new) == _grad_keys(ref)
-    for k in _grad_keys(ref):
-        U.assert_grads_close(new[k], ref[k], what=f"{case}:{k}")
+        ref.assert_equal(k, new[k])
+    assert _grad_keys(new) == _grad_keys(ref.names())
+    for k in _grad_keys(new):
+        a, b, scale = ref.pair(k, new[k])
+        U.assert_grads_close(a, b, scale=scale, what=f"{case}:{k}")
     assert (new["radii"] > 0).any()
 
 
@@ -46,9 +46,7 @@ def test_matches_golden_fixture(case):
         pytest.skip("golden fixture missing")
     G = np.load(f)
     s = scenes.scene(case)
-    for k, v in s.items():
-        if isinstance(v, np.ndarray):
-            assert np.array_equal(v, G["in_" + k]), f"scene generator drifted from the fixture ({k})"
+    U.assert_scene_matches_fixture(s, G)
     dev = torch.device("cuda")
     captured = {}
 
@@ -97,23 +95,21 @@ def test_matches_cpu_oracle(case):
 
 def test_sh_degrees_and_stride():
     """D < tensor degree: coefficients are read with stride M (quirk 13); every degree against the reference."""
-    if not ref_driver.available():
-        pytest.skip("oracle/_ref/_refC.so not present")
     s = scenes.scene("A")
     for D in (0, 1, 2, 3):
         s["D"] = D
         new = scenes.run_torch(s, U.new_rasterize, torch.device("cuda"))
-        ref = scenes.run_torch(s, U.ref_rasterize, torch.device("cuda"))
-        assert np.array_equal(new["color"], ref["color"]), D
-        U.assert_grads_close(new["g_shs"], ref["g_shs"], what=f"D={D} shs")
+        ref = refgold.reference(f"sh_degree_{D}", lambda: scenes.run_torch(s, U.ref_rasterize, torch.device("cuda")))
+        ref.assert_equal("color", new["color"], what=f"D={D} color")
+        a, b, scale = ref.pair("g_shs", new["g_shs"])
+        U.assert_grads_close(a, b, scale=scale, what=f"D={D} shs")
         assert (new["g_shs"][:, (D + 1) ** 2:, :] == 0).all()
 
 
 def test_medium_scene_bit_exact_and_sorted():
     """cfg2-shaped scene (100k Gaussians, 800x800): forward bit-exact vs the reference; the sorted list is the
-    reference's minus provably inert (Gaussian, tile) pairs, in the reference's order."""
-    if not ref_driver.available():
-        pytest.skip("oracle/_ref/_refC.so not present")
+    reference's minus provably inert (Gaussian, tile) pairs, in the reference's order (checked on a fixed selection of
+    tiles, the most crowded one included)."""
     import math
     from gaustudio_b200 import _C
     from gaustudio_b200.synthetic import build_config
@@ -121,7 +117,8 @@ def test_medium_scene_bit_exact_and_sorted():
     dev = torch.device("cuda")
     model.to(dev)
     e = torch.Tensor([])
-    for cam in cams[:2]:
+    T = ((c["W"] + 15) // 16) * ((c["H"] + 15) // 16)
+    for k, cam in enumerate(cams[:2]):
         cam.to(dev)
         with torch.no_grad():
             args = (torch.zeros(3, device=dev), model.get_attribute("xyz"), e, model.get_attribute("opacity"),
@@ -129,24 +126,28 @@ def test_medium_scene_bit_exact_and_sorted():
                     cam.full_proj_transform, math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5), c["H"], c["W"],
                     model.get_features.contiguous(), 3, cam.camera_center, False, False)
             n = _C.rasterize_gaussians(*args)
-            r = ref_driver.module().rasterize_gaussians(*args)
-        assert n[0] == r[0] > 1_000_000
+
+            def run_reference():
+                r = ref_driver.module().rasterize_gaussians(*args)
+                out = {"num_rendered": r[0], **{f"out{i}": r[i] for i in range(1, 6)}}
+                out.update(U.reference_tile_segments(ref_driver.parse_binning(r[7], r[0]),
+                                                     ref_driver.parse_image_ranges(r[8], c["W"] * c["H"], T), T, 1, 5, k))
+                return out
+            ref = refgold.reference(f"medium_view{k}", run_reference)
+        R = ref.scalar("num_rendered")
+        assert n[0] == R > 1_000_000
         for i in range(1, 6):
-            assert torch.equal(n[i], r[i]), i
+            ref.assert_equal(f"out{i}", n[i], what=f"output {i}")
         ex = _C.debug_export(c["P"], c["W"], c["H"], n[0], n[6], n[7], n[8])
-        T = ex["ranges"].shape[0]
-        dropped = U.assert_binned_list_is_culled_reference_list(
-            ex, ref_driver.parse_binning(r[7], r[0]), ref_driver.parse_image_ranges(r[8], c["W"] * c["H"], T), c["W"], c["H"],
-            c["P"])
-        assert 0 < dropped < r[0] // 2 and ex["num_binned"] == r[0] - dropped
+        U.assert_binned_list_is_culled_reference_list(ex, ref.array("seg_list"), ref.array("seg_ranges"), c["W"], c["H"],
+                                                      c["P"], tiles=ref.array("seg_tiles"))
+        assert 0 < R - ex["num_binned"] < R // 2
 
 
 def test_sparse_and_dense_projection_ctas_match_reference():
     """A scene whose projection CTAs are a mix of dense ones (everything visible) and sparse ones (most Gaussians
     behind the camera or far off screen, some off-screen centres whose splats still reach the image) stays
     bit-identical to the compiled reference; gradients within 1e-3."""
-    if not ref_driver.available():
-        pytest.skip("oracle/_ref/_refC.so not present")
     s = dict(scenes.scene("D"))
     rng = np.random.RandomState(21)
     P = s["means3D"].shape[0]
@@ -159,9 +160,11 @@ def test_sparse_and_dense_projection_ctas_match_reference():
     s["means3D"], s["scales"] = xyz, sc
     dev = torch.device("cuda")
     new = scenes.run_torch(s, U.new_rasterize, dev)
-    ref = scenes.run_torch(s, U.ref_rasterize, dev)
-    assert 0.2 < (ref["radii"] > 0).mean() < 0.8
+    ref = refgold.reference("sparse_dense", lambda: scenes.run_torch(s, U.ref_rasterize, dev))
     for k in FWD + ("radii",):
-        assert np.array_equal(new[k], ref[k]), f"{k} not bit-identical to the reference"
-    for k in _grad_keys(ref):
-        U.assert_grads_close(new[k], ref[k], what=f"sparse:{k}")
+        ref.assert_equal(k, new[k])
+    assert 0.2 < (new["radii"] > 0).mean() < 0.8
+    assert _grad_keys(new) == _grad_keys(ref.names())
+    for k in _grad_keys(new):
+        a, b, scale = ref.pair(k, new[k])
+        U.assert_grads_close(a, b, scale=scale, what=f"sparse:{k}")

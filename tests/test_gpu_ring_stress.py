@@ -67,14 +67,14 @@ def _same(a, b, what):
                 assert abs(x - y) <= 1e-5 * max(abs(x), 1e-12), (what, k, x, y)
 
 
-def test_tma_gather4_staging_reproduces_default_build():
-    """GSR_FWD_TMA=1: the compositing forward stages its record batches with TMA tile::gather4 copies (four 48-byte rows
-    per instruction through a tensor map over the splat array) instead of per-record LDGSTS copies.  Same pixels, bit
-    for bit -- also on the one-stage ring.  (It is opt-in because it measures slower: DESIGN.md 3.2.)"""
+def test_tma_bulk_staging_reproduces_default_build():
+    """GSR_FWD_TMA=1: the compositing forward stages its record batches with TMA bulk copies (one 48-byte cp.async.bulk
+    per record, completing on the stage's mbarrier) instead of per-record LDGSTS copies.  Same pixels, bit for bit --
+    also on the one-stage ring."""
     ref = _run(None)
-    _same(ref, _run(None, GSR_FWD_TMA="1"), "with TMA gather4 staging")
+    _same(ref, _run(None, GSR_FWD_TMA="1"), "with TMA bulk-copy staging")
     if os.path.exists(STRESS):
-        _same(ref, _run(STRESS, GSR_FWD_TMA="1"), "with TMA gather4 staging on the one-stage ring")
+        _same(ref, _run(STRESS, GSR_FWD_TMA="1"), "with TMA bulk-copy staging on the one-stage ring")
 
 
 def test_two_pixels_per_lane_backward_matches_default():

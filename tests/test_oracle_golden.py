@@ -1,5 +1,5 @@
 """Pins the CPU oracle: oracle vs the golden tensors the unmodified reference CUDA extension produced on a
-B200 (tests/golden/ref_case_*.npz, generator tests/golden/make_golden_ref.py).  Runs without a GPU."""
+GPU (tests/golden/ref_case_*.npz, generator tests/golden/make_golden_ref.py).  Runs without a GPU."""
 import os
 
 import numpy as np
@@ -18,9 +18,7 @@ def test_oracle_reproduces_reference_outputs(case):
         pytest.skip("golden fixture missing (generate on the GPU box)")
     G = np.load(f)
     s = scenes.scene(case)
-    for k, v in s.items():
-        if isinstance(v, np.ndarray):
-            assert np.array_equal(v, G["in_" + k]), f"scene generator drifted from the fixture ({k})"
+    U.assert_scene_matches_fixture(s, G)
     orc = U.oracle_run(s)
     assert abs(orc["num_rendered"] - int(G["ref_num_rendered"])) <= 2
     assert (orc["radii"] != G["ref_radii"]).mean() < 1e-3

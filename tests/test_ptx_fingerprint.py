@@ -29,7 +29,7 @@ FP_OP = re.compile(r"^\s*(?:@%p\d+\s+)?((?:fma|mul|add|sub|div|rcp|sqrt|rsqrt|ex
 def _fingerprints():
     out = {}
     for src, frag in KERNELS:
-        ptx = subprocess.run([NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17",
+        ptx = subprocess.run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17",
                               "--expt-relaxed-constexpr", "--extended-lambda", "-I", os.path.join(ROOT, "include"),
                               "-ptx", "-o", "/dev/stdout", os.path.join(CSRC, src)],
                              check=True, capture_output=True, text=True).stdout

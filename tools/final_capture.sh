@@ -1,5 +1,5 @@
 #!/bin/bash
-# End-of-round evidence run (1 x B200), most important first: GPU test suite, both bench arms, cfg5, training step, the
+# End-of-round evidence run (1 x H100), most important first: GPU test suite, both bench arms, cfg5, training step, the
 # launch list of bench.py, ncu --set full of one steady-state step, then a repeat loop of the binding tests and the same
 # suite / benches with the exact-mode speculation off (GSR_SPECULATE=0) for comparison.  (The r2c capture in profiles/
 # was taken when the experimental cluster scan was still a run-time default: its `off` leg also had GSR_SCAN_CLUSTER=0.)

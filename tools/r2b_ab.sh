@@ -1,7 +1,7 @@
 #!/bin/bash
 # NOTE: since the end of round 2 the cluster tile scan is compiled only into the `cluster_scan` variant (python tools/build_variants.py
 # cluster_scan; run with GSR_LIB=gaustudio_b200/variants/libgsr_cluster_scan.so): with the default library GSR_SCAN_CLUSTER is ignored.
-# One-call A/B of the late round-2 changes (1 x B200): GPU tests first, then bench.py under the knobs
+# One-call A/B of the late round-2 changes (1 x H100): GPU tests first, then bench.py under the knobs
 #   GSR_SCAN_CLUSTER (8-CTA cluster scan vs the single-CTA scan), GSR_SPECULATE (exact-mode speculation: drop-in leg),
 #   GSR_CARVEOUT (uniform shared-memory carveout), GSR_SKIP_CROWDED (cost of the two empty crowded-tier launches).
 mkdir -p gpurun_out

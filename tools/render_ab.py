@@ -1,5 +1,5 @@
 """A/B of the compositing-kernel variants selected by environment variables read once per process (GSR_BWD_NSUB = pixels
-per lane of the backward: 1 or 2; GSR_FWD_TMA=1 = TMA gather4 staging in the forward), one subprocess per variant.
+per lane of the backward: 1 or 2; GSR_FWD_TMA=1 = TMA bulk-copy staging in the forward), one subprocess per variant.
 (Up to commit a9bd034 the backward also had 4 / 8 pixels per lane and a second occupancy target per variant --
 `GSR_BWD_MINB`; those measurements are in profiles/r2_ab_bwd_variants.json.)  For each variant: forward
 outputs must be BIT-IDENTICAL to the unmodified reference extension (oracle/_ref) and the gradients within 1e-3
