@@ -324,7 +324,7 @@ def rasterize_gaussians_fused_backward(background, means3D, radii, f_dc, f_rest,
     M = 1 + (f_rest.numel() // (3 * P) if f_rest.numel() else 0)
     d_m3 = torch.empty(P, 3, **fopt); d_m2 = torch.empty(P, 3, **fopt); d_op = torch.empty_like(opacity_logits)
     d_dc = torch.empty_like(f_dc); d_rest = torch.empty_like(f_rest); d_sc = torch.empty(P, 3, **fopt)
-    d_rot = torch.empty(P, 4, **fopt); d_col = torch.empty(P, 3, **fopt); d_cov = torch.empty(P, 6, **fopt)
+    d_rot = torch.empty(P, 4, **fopt)
     means3D = _f32(means3D, dev, "means3D"); opacity_logits = _f32(opacity_logits, dev, "opacity")
     log_scales = _f32(log_scales, dev, "scales"); raw_rotations = _f32(raw_rotations, dev, "rotations")
     viewmatrix = _f32(viewmatrix, dev, "viewmatrix"); projmatrix = _f32(projmatrix, dev, "projmatrix")
@@ -337,8 +337,8 @@ def rasterize_gaussians_fused_backward(background, means3D, radii, f_dc, f_rest,
                                   _ptr(f_rest), _ptr(opacity_logits), _ptr(log_scales), float(scale_modifier),
                                   _ptr(raw_rotations), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), float(tan_fovx),
                                   float(tan_fovy), _ptr(radii), _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imageBuffer),
-                                  _ptr(gc), _ptr(gd), _ptr(gm), _ptr(go), _ptr(d_m2), _ptr(d_op), _ptr(d_col), _ptr(d_m3),
-                                  _ptr(d_cov), _ptr(d_dc), _ptr(d_rest), _ptr(d_sc), _ptr(d_rot), int(bool(debug)),
+                                  _ptr(gc), _ptr(gd), _ptr(gm), _ptr(go), _ptr(d_m2), _ptr(d_op), None, _ptr(d_m3),
+                                  None, _ptr(d_dc), _ptr(d_rest), _ptr(d_sc), _ptr(d_rot), int(bool(debug)),
                                   stream.cuda_stream)
     if rc < 0:
         raise RuntimeError("gsr_backward_fused failed: " + _lib.last_error())

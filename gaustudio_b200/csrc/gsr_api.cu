@@ -462,6 +462,10 @@ static int backward_impl(int fused, const float* f_dc, const float* f_rest, cons
   if (P <= 0) return 0;
   if (!geom_buffer || !image_buffer || (!binning_buffer && R > 0)) { g_err = "gsr_backward: missing state buffers"; return -1; }
   if (!background) { g_err = "gsr_backward: background must be a device pointer (backward.cu:586 reads it)"; return -1; }
+  if (!cov3D_precomp && (!scales || !rotations)) {  // the backward recomputes cov3D from them
+    g_err = "gsr_backward: scales and rotations are required when cov3D_precomp is NULL";
+    return -1;
+  }
   const int gx = (width + TILE_X - 1) / TILE_X, gy = (height + TILE_Y - 1) / TILE_Y;
   GeomView g = carve_geom(aligned_base(geom_buffer), P);
   ImageView im = carve_image(aligned_base(image_buffer), width, height);

@@ -88,7 +88,9 @@ int gsr_backward(int P, int D, int M, int64_t R, const float* background, int wi
  * model's RAW attributes instead -- log_scales[P,3], raw_rotations[P,4], opacity_logits[P], f_dc[P,1,3],
  * f_rest[P,M-1,3] -- and apply the activations inside the projection kernel; the backward returns gradients
  * w.r.t. the raw attributes (dL_dlog_scale, dL_draw_rot, dL_dopacity_logit, dL_df_dc, dL_df_rest).  Everything
- * else is identical to gsr_forward / gsr_backward; the opaque buffers are interchangeable. */
+ * else is identical to gsr_forward / gsr_backward; the opaque buffers are interchangeable.
+ * gsr_backward_fused: dL_dcolor[P,3] and dL_dcov3D[P,6] (the gradients w.r.t. the intermediate colours and 3D
+ * covariances) may be NULL; they are not written then. */
 int64_t gsr_forward_fused(gsr_alloc_fn geometry_alloc, void* geometry_user, gsr_alloc_fn binning_alloc,
                           void* binning_user, gsr_alloc_fn image_alloc, void* image_user, int P, int D, int M,
                           const float* background, int width, int height, const float* means3D, const float* f_dc,
