@@ -69,13 +69,14 @@ def assert_images_close(a, b, atol=1e-4, outlier_frac=0.0, what=""):
     assert frac <= outlier_frac, f"{what}: {frac:.2e} of pixels beyond {atol} (max {err.max():.3e})"
 
 
-def reference_tile_segments(point_list, ranges, T, n_crowded, n_random, seed):
-    """A fixed selection of tiles of the reference's sorted list (the n_crowded most crowded ones and n_random other
-    non-empty ones) with their segments of the list: {seg_tiles, seg_ranges, seg_list}, seg_ranges indexing seg_list."""
+def reference_tile_segments(point_list, ranges, T, n_crowded, n_random, seed, extra=()):
+    """A fixed selection of tiles of the reference's sorted list (the n_crowded most crowded ones, the tiles `extra` and
+    n_random other non-empty ones) with their segments of the list: {seg_tiles, seg_ranges, seg_list}, seg_ranges
+    indexing seg_list."""
     rg = np.asarray(ranges.cpu() if torch.is_tensor(ranges) else ranges).astype(np.int64).reshape(-1, 2)[:T]
     pl = np.asarray(point_list.cpu() if torch.is_tensor(point_list) else point_list)
     n = rg[:, 1] - rg[:, 0]
-    crowded = np.argsort(-n, kind="stable")[:n_crowded]
+    crowded = np.union1d(np.argsort(-n, kind="stable")[:n_crowded], np.asarray(extra, np.int64))
     rest = np.setdiff1d(np.nonzero(n)[0], crowded)
     tiles = np.sort(np.concatenate([crowded, np.random.RandomState(seed).choice(rest, n_random, replace=False)]))
     segs = [pl[rg[t, 0]:rg[t, 1]] for t in tiles]

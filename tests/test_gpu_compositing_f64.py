@@ -47,7 +47,8 @@ def view_scene(kind, W, H, seed):
     rng = np.random.RandomState(seed)
     cam = scenes.camera(W, H, 50.0)
     tx, ty = math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5)
-    P = {"deep": 700, "saturating": 400, "partial": max(60, W * H // 60), "offscreen_thin": 600, "equal": 400}[kind]
+    P = {"deep": 700, "saturating": 400, "partial": max(60, W * H // 60), "offscreen_thin": 600, "equal": 400,
+         "wide": 1200}[kind]
     z = rng.uniform(1.5, 4.0, P)
     u, v = rng.uniform(-1, 1, P) * tx, rng.uniform(-1, 1, P) * ty
     s = 0.025 * z[:, None] * np.exp(0.3 * rng.randn(P, 3))
@@ -64,6 +65,12 @@ def view_scene(kind, W, H, seed):
         op = np.where(rng.rand(P) < 0.5, rng.uniform(0.995, 1.0, P), rng.uniform(0.85, 0.995, P))
         s = 0.05 * z[:, None] * np.exp(0.3 * rng.randn(P, 3))
         bg = np.array([1.0, 1.0, 1.0])
+    elif kind == "wide":
+        # small splats (sigma ~ 2-5 px) all over an image of several tile-scan rounds (8192 tiles each)
+        s = 0.0018 * z[:, None] * np.exp(0.3 * rng.randn(P, 3))
+        # and a few wider ones on the centre of the image, where the one-block upstream pattern lies
+        u[:8], v[:8] = _pix_to_u(W / 2 + 4 * rng.randn(8), W, tx), _pix_to_u(H / 2 + 2 * rng.randn(8), H, ty)
+        s[:8] *= 3
     elif kind == "offscreen_thin":
         half = P // 2
         # centres beyond the image edges (inside the lateral clamp), wide enough to reach the screen
@@ -97,6 +104,8 @@ SCENES = {
     "partial250x170": lambda: view_scene("partial", 250, 170, 4),
     "offscreen_thin": lambda: view_scene("offscreen_thin", 64, 48, 5),
     "equal": lambda: view_scene("equal", 64, 48, 6),
+    "wide3840x2160": lambda: view_scene("wide", 3840, 2160, 7),   # four rounds, the last one partial
+    "wide2561x1441": lambda: view_scene("wide", 2561, 1441, 8),   # two rounds, partial tiles on both edges
 }
 
 
@@ -278,6 +287,13 @@ def test_accumulator_matches_f64_reference(key):
         disc = torch.sqrt((tr * tr / 4 - det).clamp(min=0))
         ratio = (tr / 2 + disc) / (tr / 2 - disc).clamp(min=1e-30)
         assert int((live & (ratio > 100) & (co[:, 1].abs() > 0.2 * co[:, 0].abs())).sum()) >= 20
+    if key.startswith("wide"):
+        # Gaussians reached by the upstream in every round of the tile scan
+        gx = (fr.W + 15) // 16
+        T = gx * ((fr.H + 15) // 16)
+        cov = ref.covered.reshape(fr.H, fr.W).nonzero()
+        hit = set(((cov[:, 0] // 16) * gx + cov[:, 1] // 16).div(8192, rounding_mode="floor").tolist())
+        assert T > 8192 and hit == set(range((T + 8191) // 8192)), (T, hit)
     if key == "equal":
         d = fr.ex["depths"][fr.radii.cpu() > 0]
         assert len(d) - len(torch.unique(d)) >= 50
