@@ -4,6 +4,7 @@ returned tuples -- implemented on top of the C ABI of libgsr_b200.so (include/gs
 PyTorch is only the owner of device memory and of the current stream here.
 """
 import ctypes as C
+import math
 import threading
 
 import torch
@@ -190,9 +191,10 @@ _ALLOC = _lib.ALLOC_FN(_alloc)
 
 def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                         viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
-                        prefiltered, debug, _fused=None):
+                        prefiltered, debug, _fused=None, _kernel_size=None):
     """_fused=(f_dc, f_rest): fused-activation variant (gsr_forward_fused): `opacity`, `scales`, `rotations` are
-    then the model's RAW attributes and `sh` / `colors` / `cov3D_precomp` are ignored."""
+    then the model's RAW attributes and `sh` / `colors` / `cov3D_precomp` are ignored.
+    _kernel_size: the Mip-Splatting projection (gsr_forward_mip); see rasterize_gaussians_mip."""
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")  # rasterize_points.cu:57-59
     if not means3D.is_cuda:
@@ -246,7 +248,12 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
         tail = (float(tan_fovx), float(tan_fovy), int(bool(prefiltered)), _ptr(out_color), _ptr(out_depth),
                 _ptr(out_median), _ptr(out_opacity), _ptr(radii), int(bool(debug)), int(cap),
                 host.data_ptr() if host is not None else None, stream.cuda_stream)
-        if _fused is None:
+        if _kernel_size is not None:
+            r = L.gsr_forward_mip(_ALLOC, 1, _ALLOC, 2, _ALLOC, 3, P, int(degree), M, _ptr(background), W, H,
+                                  _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(opacity), _ptr(scales),
+                                  float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(viewmatrix),
+                                  _ptr(projmatrix), _ptr(campos), *tail[:-1], float(_kernel_size), tail[-1])
+        elif _fused is None:
             r = L.gsr_forward(_ALLOC, 1, _ALLOC, 2, _ALLOC, 3, P, int(degree), M, _ptr(background), W, H,
                               _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(opacity), _ptr(scales),
                               float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(viewmatrix),
@@ -282,7 +289,8 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
 def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp,
                                  viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, dL_dout_depth,
                                  dL_dout_median_depth, dL_dout_final_opacity, sh, degree, campos, geomBuffer, R,
-                                 binningBuffer, imageBuffer, debug):
+                                 binningBuffer, imageBuffer, debug, _mip=None):
+    """_mip=(opacities, kernel_size): the backward of the Mip-Splatting projection (gsr_backward_mip)."""
     L = _lib.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -305,16 +313,20 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         radii = radii.contiguous()
         with _on_device(dev):
             stream = torch.cuda.current_stream(dev)
-            rc = L.gsr_backward(P, int(degree), M, int(R), _ptr(background), W, H, _ptr(means3D), _ptr(sh),
-                                _ptr(colors), _ptr(scales), float(scale_modifier), _ptr(rotations),
-                                _ptr(cov3D_precomp), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), float(tan_fovx),
-                                float(tan_fovy), _ptr(radii), _ptr(geomBuffer), _ptr(binningBuffer),
-                                _ptr(imageBuffer), _ptr(gc), _ptr(gd), _ptr(gm), _ptr(go), _ptr(dL_dmeans2D), None,
-                                _ptr(dL_dopacity), _ptr(dL_dcolors), None, _ptr(dL_dmeans3D), _ptr(dL_dcov3D),
-                                _ptr(dL_dsh), _ptr(dL_dscales), _ptr(dL_drotations), int(bool(debug)),
-                                stream.cuda_stream)
+            args = (P, int(degree), M, int(R), _ptr(background), W, H, _ptr(means3D), _ptr(sh), _ptr(colors),
+                    _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(viewmatrix),
+                    _ptr(projmatrix), _ptr(campos), float(tan_fovx), float(tan_fovy), _ptr(radii), _ptr(geomBuffer),
+                    _ptr(binningBuffer), _ptr(imageBuffer), _ptr(gc), _ptr(gd), _ptr(gm), _ptr(go),
+                    _ptr(dL_dmeans2D), None, _ptr(dL_dopacity), _ptr(dL_dcolors), None, _ptr(dL_dmeans3D),
+                    _ptr(dL_dcov3D), _ptr(dL_dsh), _ptr(dL_dscales), _ptr(dL_drotations), int(bool(debug)))
+            if _mip is None:
+                rc = L.gsr_backward(*args, stream.cuda_stream)
+            else:
+                opac = _f32(_mip[0], dev, "opacities")
+                rc = L.gsr_backward_mip(*args, _ptr(opac), float(_mip[1]), stream.cuda_stream)
         if rc < 0:
-            raise RuntimeError("gsr_backward failed: " + _lib.last_error())
+            raise RuntimeError(("gsr_backward failed: " if _mip is None else "gsr_backward_mip failed: ")
+                               + _lib.last_error())
     return dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations
 
 
@@ -352,6 +364,105 @@ def rasterize_gaussians_fused_backward(background, means3D, radii, f_dc, f_rest,
     if rc < 0:
         raise RuntimeError("gsr_backward_fused failed: " + _lib.last_error())
     return d_m2, d_op, d_m3, d_dc, d_rest, d_sc, d_rot
+
+
+# ---- Mip-Splatting: gsr_forward_mip / gsr_backward_mip / gsr_mip_filter3d (include/gsr.h) -----------------------------
+def _check_kernel_size(kernel_size):
+    k = float(kernel_size)
+    if not (k >= 0.0 and k < float("inf")):
+        raise ValueError(f"kernel_size must be finite and >= 0, got {kernel_size!r}")
+    return k
+
+
+def rasterize_gaussians_mip(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
+                            viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
+                            prefiltered, debug, kernel_size):
+    """rasterize_gaussians with the 2D Mip filter of width `kernel_size` in the projection (gsr_forward_mip): the
+    splats' opacity is opacity * coef and their covariance cov2D + kernel_size I.  Same returned tuple."""
+    return rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
+                               viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
+                               prefiltered, debug, _kernel_size=_check_kernel_size(kernel_size))
+
+
+def rasterize_gaussians_mip_backward(background, means3D, radii, colors, opacities, scales, rotations, scale_modifier,
+                                     cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color,
+                                     dL_dout_depth, dL_dout_median_depth, dL_dout_final_opacity, sh, degree, campos,
+                                     geomBuffer, R, binningBuffer, imageBuffer, debug, kernel_size):
+    """Backward of rasterize_gaussians_mip (gsr_backward_mip): the tuple of rasterize_gaussians_backward, with the
+    opacity gradient w.r.t. the input `opacities`."""
+    return rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, scale_modifier,
+                                        cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color,
+                                        dL_dout_depth, dL_dout_median_depth, dL_dout_final_opacity, sh, degree, campos,
+                                        geomBuffer, R, binningBuffer, imageBuffer, debug,
+                                        _mip=(opacities, _check_kernel_size(kernel_size)))
+
+
+def debug_projection_backward_mip(means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations,
+                                  cov3D_precomp, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, image_height,
+                                  image_width, degree, radii, geomBuffer, accum, kernel_size):
+    """The Mip projection backward alone on caller-chosen per-Gaussian sums `accum` [P,12] (tests; see
+    gsr_debug_projection_backward_mip in include/gsr.h).  geomBuffer holds a rasterize_gaussians_mip forward of the same
+    Gaussians and camera.  -> dict of every output (mean2D, conic, opacity, color, depth, mean3D, cov3D, shs, scale,
+    rot), each fully written by the kernel."""
+    L = _lib.lib()
+    dev = means3D.device
+    P, H, W = means3D.size(0), int(image_height), int(image_width)
+    M = shs.size(1) if shs is not None and shs.numel() != 0 else 0
+    means3D, shs, colors_precomp = _f32(means3D, dev, "means3D"), _f32(shs, dev, "shs"), _f32(colors_precomp, dev, "colors")
+    opacities, scales = _f32(opacities, dev, "opacities"), _f32(scales, dev, "scales")
+    rotations, cov3D_precomp = _f32_rot(rotations, dev, "rotations"), _f32(cov3D_precomp, dev, "cov3D_precomp")
+    viewmatrix, projmatrix = _f32(viewmatrix, dev, "viewmatrix"), _f32(projmatrix, dev, "projmatrix")
+    campos, radii = _f32(campos, dev, "campos"), radii.contiguous()
+    e = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+    o = dict(mean2D=e(P, 3), conic=e(P, 4), opacity=e(P), color=e(P, 3), depth=e(P), mean3D=e(P, 3), cov3D=e(P, 6),
+             shs=e(P, M, 3), scale=e(P, 3), rot=e(P, 4))
+    acc = accum.to(dev, torch.float32).contiguous()
+    with _on_device(dev):
+        rc = L.gsr_debug_projection_backward_mip(
+            P, int(degree), M, W, H, _ptr(means3D), _ptr(shs), _ptr(colors_precomp), _ptr(opacities), _ptr(scales),
+            float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(viewmatrix), _ptr(projmatrix),
+            _ptr(campos), float(tan_fovx), float(tan_fovy), _ptr(radii), _ptr(geomBuffer), _ptr(acc), _ptr(o["mean2D"]),
+            _ptr(o["conic"]), _ptr(o["opacity"]), _ptr(o["color"]), _ptr(o["depth"]), _ptr(o["mean3D"]),
+            _ptr(o["cov3D"]), _ptr(o["shs"]), _ptr(o["scale"]), _ptr(o["rot"]), _check_kernel_size(kernel_size), 0,
+            torch.cuda.current_stream(dev).cuda_stream)
+    if rc < 0:
+        raise RuntimeError("gsr_debug_projection_backward_mip failed: " + _lib.last_error())
+    return o
+
+
+def mip_camera_records(cameras, device):
+    """[C,16] float32 camera records of gsr_mip_filter3d: R (row-major Camera.R), T, fx, fy, width, height."""
+    rows = []
+    for c in cameras:
+        fx = c.image_width / (2.0 * math.tan(c.FoVx * 0.5))
+        fy = c.image_height / (2.0 * math.tan(c.FoVy * 0.5))
+        rows.append([float(v) for v in torch.as_tensor(c.R, dtype=torch.float64).reshape(9)] +
+                    [float(v) for v in torch.as_tensor(c.T, dtype=torch.float64).reshape(3)] +
+                    [fx, fy, float(c.image_width), float(c.image_height)])
+    return torch.tensor(rows, dtype=torch.float32).reshape(-1, 16).to(device)
+
+
+def mip_filter3d(means3D, cameras):
+    """Mip-Splatting's 3D smoothing filter [P] over `cameras` (Camera objects, or a [C,16] tensor of
+    mip_camera_records) in one device pass (gsr_mip_filter3d).  Raises ValueError when no camera sees any Gaussian
+    (one host synchronisation to read the count)."""
+    if not means3D.is_cuda:
+        raise RuntimeError("gaustudio_b200 runs on CUDA (sm_90a) only; means3D must be a CUDA tensor")
+    dev = means3D.device
+    P = means3D.size(0)
+    recs = cameras if torch.is_tensor(cameras) else mip_camera_records(cameras, dev)
+    recs = _f32(recs, dev, "cameras")
+    means3D = _f32(means3D, dev, "means3D")
+    out = torch.empty(P, dtype=torch.float32, device=dev)
+    scratch = torch.empty(3, dtype=torch.int32, device=dev)
+    with _on_device(dev):
+        rc = _lib.lib().gsr_mip_filter3d(P, _ptr(means3D), int(recs.numel() // 16), _ptr(recs), _ptr(out),
+                                         _ptr(scratch), torch.cuda.current_stream(dev).cuda_stream)
+    if rc < 0:
+        raise RuntimeError("gsr_mip_filter3d failed: " + _lib.last_error())
+    if P == 0 or int(scratch[2]) == 0:
+        raise ValueError("compute_3D_filter: no camera sees any Gaussian")
+    return out
 
 
 def mark_visible(means3D, viewmatrix, projmatrix):

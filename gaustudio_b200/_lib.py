@@ -61,6 +61,13 @@ SIGNATURES = {
     "gsr_debug_accumulator": (_I, [_I, _P, _P, _P]),
     "gsr_debug_projection_backward": (_I, [_I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _F, _P, _P, _P, _P, _P,
                                            _F, _F, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P]),
+    "gsr_forward_mip": (_L, [ALLOC_FN, _P, ALLOC_FN, _P, ALLOC_FN, _P, _I, _I, _I, _P, _I, _I, _P, _P, _P, _P, _P, _F, _P,
+                             _P, _P, _P, _P, _F, _F, _I, _P, _P, _P, _P, _P, _I, _L, _P, _F, _P]),
+    "gsr_backward_mip": (_I, [_I, _I, _I, _L, _P, _I, _I, _P, _P, _P, _P, _F, _P, _P, _P, _P, _P, _F, _F, _P, _P, _P, _P,
+                              _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _F, _P]),
+    "gsr_debug_projection_backward_mip": (_I, [_I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _F, _P, _P, _P, _P, _P, _F, _F,
+                                               _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _F, _I, _P]),
+    "gsr_mip_filter3d": (_I, [_I, _P, _I, _P, _P, _P, _P]),
 }
 
 _lib = None

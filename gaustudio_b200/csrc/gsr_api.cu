@@ -342,6 +342,8 @@ struct FwdHost {
   int64_t r_capacity;  // > 0: pipelined mode
   int64_t* r_host;
   cudaStream_t stream;
+  bool mip;  // gsr_forward_mip: the 2D Mip filter of width kernel_size replaces the 0.3 dilation
+  float kernel_size;
 };
 // what a backward takes besides the kernels' arguments (BwdArgs)
 struct BwdHost {
@@ -353,6 +355,9 @@ struct BwdHost {
   const float* accum;
   int debug;
   cudaStream_t stream;
+  bool mip;  // gsr_backward_mip: the backward of the Mip projection, which needs the input opacities
+  float kernel_size;
+  const float* opacities;
 };
 
 const char* forward_error(const FwdArgs& a) {
@@ -390,7 +395,11 @@ bool first_half(const FwdArgs& a, const FwdHost& h, GeomView g, ImageView im, un
   const int T = a.gx * a.gy;
   if (!check(cudaMemsetAsync(im.tile_count, 0, sizeof(uint32_t) * T * SUBBINS, h.stream), "memset tile_count")) return false;
   launch_high_priority(k_init_header, dim3(1), dim3(1), 0, h.stream, im.hdr, cap);
-  { Prof pf(kPreprocessFwd, h.stream); launch_preprocess_fwd(a, g, im, h.stream); }
+  {
+    Prof pf(kPreprocessFwd, h.stream);
+    if (h.mip) launch_mip_preprocess_fwd(a, g, im, h.kernel_size, h.stream);
+    else launch_preprocess_fwd(a, g, im, h.stream);
+  }
   if (!stage_ok(h.debug, h.stream, "preprocess_fwd")) return false;
   { Prof pf(kTileScan, h.stream); launch_tile_scan(im, T, h.stream); }
   return stage_ok(h.debug, h.stream, "tile_scan");
@@ -491,12 +500,20 @@ int backward_impl(BwdArgs& a, const BwdHost& h) {
   a.focal_x = a.W / (2.0f * a.tan_fovx);
   if (a.fused) choose_sh_staging(a, {a.f_dc, a.f_rest, a.dL_df_dc, a.dL_df_rest});
   else choose_sh_staging(a, {a.shs, a.dL_dsh});
-  { Prof pf(kPreprocessBwd, h.stream); launch_preprocess_bwd(a, g, h.stream); }
+  {
+    Prof pf(kPreprocessBwd, h.stream);
+    if (h.mip) launch_mip_preprocess_bwd(a, g, h.opacities, h.kernel_size, h.stream);
+    else launch_preprocess_bwd(a, g, h.stream);
+  }
   return stage_ok(h.debug, h.stream, "preprocess_bwd") ? 0 : -1;
 }
 }  // namespace
 
 void set_last_error(const char* msg) { g_err = msg; }
+
+namespace {
+bool mip_kernel_size_ok(float k) { return std::isfinite(k) && k >= 0.f; }
+}  // namespace
 
 }  // namespace gsr
 
@@ -579,6 +596,30 @@ int gsr_backward(int P, int D, int M, int64_t R, const float* background, int wi
   return backward_impl(a, h);
 }
 
+int64_t gsr_forward_mip(gsr_alloc_fn geometry_alloc, void* geometry_user, gsr_alloc_fn binning_alloc, void* binning_user,
+                        gsr_alloc_fn image_alloc, void* image_user, int P, int D, int M, const float* background,
+                        int width, int height, const float* means3D, const float* shs, const float* colors_precomp,
+                        const float* opacities, const float* scales, float scale_modifier, const float* rotations,
+                        const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix,
+                        const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
+                        float* out_depth, float* out_median_depth, float* out_opacity, int* radii, int debug,
+                        int64_t r_capacity, int64_t* r_host, float kernel_size, void* stream) {
+  if (!mip_kernel_size_ok(kernel_size)) { g_err = "gsr_forward_mip: kernel_size must be finite and >= 0"; return -1; }
+  FwdArgs a{};
+  a.P = P; a.D = D; a.M = M; a.W = width; a.H = height; a.prefiltered = prefiltered; a.radii_out = radii;
+  a.means3D = means3D; a.shs = shs; a.colors_precomp = colors_precomp; a.opacities = opacities;
+  a.scales = scales; a.rotations = rotations; a.cov3D_precomp = cov3D_precomp;
+  a.view = viewmatrix; a.proj = projmatrix; a.campos = cam_pos;
+  a.scale_modifier = scale_modifier; a.tan_fovx = tan_fovx; a.tan_fovy = tan_fovy;
+  FwdHost h{};
+  h.geometry_alloc = geometry_alloc; h.geometry_user = geometry_user; h.binning_alloc = binning_alloc;
+  h.binning_user = binning_user; h.image_alloc = image_alloc; h.image_user = image_user;
+  h.out_color = out_color; h.out_depth = out_depth; h.out_median_depth = out_median_depth; h.out_opacity = out_opacity;
+  h.debug = debug; h.r_capacity = r_capacity; h.r_host = r_host; h.stream = (cudaStream_t)stream;
+  h.mip = true; h.kernel_size = kernel_size;
+  return forward_impl(a, h);
+}
+
 int gsr_backward_fused(int P, int D, int M, int64_t R, const float* background, int width, int height,
                        const float* means3D, const float* f_dc, const float* f_rest, const float* opacity_logits,
                        const float* log_scales, float scale_modifier, const float* raw_rotations,
@@ -601,6 +642,34 @@ int gsr_backward_fused(int P, int D, int M, int64_t R, const float* background, 
   h.dL_dpix = dL_dpix; h.dL_dpix_depth = dL_dpix_depth; h.dL_dpix_median_depth = dL_dpix_median_depth;
   h.dL_dpix_final_opacity = dL_dpix_final_opacity; h.background = background; h.debug = debug;
   h.stream = (cudaStream_t)stream;
+  return backward_impl(a, h);
+}
+
+int gsr_backward_mip(int P, int D, int M, int64_t R, const float* background, int width, int height,
+                     const float* means3D, const float* shs, const float* colors_precomp, const float* scales,
+                     float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
+                     const float* projmatrix, const float* campos, float tan_fovx, float tan_fovy, const int* radii,
+                     char* geom_buffer, char* binning_buffer, char* image_buffer, const float* dL_dpix,
+                     const float* dL_dpix_depth, const float* dL_dpix_median_depth, const float* dL_dpix_final_opacity,
+                     float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_ddepth,
+                     float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, int debug,
+                     const float* opacities, float kernel_size, void* stream) {
+  if (!mip_kernel_size_ok(kernel_size)) { g_err = "gsr_backward_mip: kernel_size must be finite and >= 0"; return -1; }
+  if (P > 0 && !opacities) { g_err = "gsr_backward_mip: opacities are required"; return -1; }
+  BwdArgs a{};
+  a.P = P; a.D = D; a.M = M; a.W = width; a.H = height; a.radii = radii;
+  a.means3D = means3D; a.shs = shs; a.colors_precomp = colors_precomp; a.scales = scales; a.rotations = rotations;
+  a.cov3D_precomp = cov3D_precomp; a.view = viewmatrix; a.proj = projmatrix; a.campos = campos;
+  a.scale_modifier = scale_modifier; a.tan_fovx = tan_fovx; a.tan_fovy = tan_fovy;
+  a.dL_dmean2D = dL_dmean2D; a.dL_dconic = dL_dconic; a.dL_dopacity = dL_dopacity; a.dL_dcolor = dL_dcolor;
+  a.dL_ddepth = dL_ddepth; a.dL_dmean3D = dL_dmean3D; a.dL_dcov3D = dL_dcov3D; a.dL_dsh = dL_dsh;
+  a.dL_dscale = dL_dscale; a.dL_drot = dL_drot;
+  BwdHost h{};
+  h.R = R; h.geom_buffer = geom_buffer; h.binning_buffer = binning_buffer; h.image_buffer = image_buffer;
+  h.dL_dpix = dL_dpix; h.dL_dpix_depth = dL_dpix_depth; h.dL_dpix_median_depth = dL_dpix_median_depth;
+  h.dL_dpix_final_opacity = dL_dpix_final_opacity; h.background = background; h.debug = debug;
+  h.stream = (cudaStream_t)stream;
+  h.mip = true; h.kernel_size = kernel_size; h.opacities = opacities;
   return backward_impl(a, h);
 }
 
@@ -749,6 +818,34 @@ int gsr_debug_projection_backward(int fused, int P, int D, int M, int width, int
   }
   BwdHost h{};
   h.geom_buffer = geom_buffer; h.accum = accum; h.debug = debug; h.stream = (cudaStream_t)stream;
+  return backward_impl(a, h);
+}
+
+int gsr_debug_projection_backward_mip(int P, int D, int M, int width, int height, const float* means3D,
+                                      const float* shs, const float* colors_precomp, const float* opacities,
+                                      const float* scales, float scale_modifier, const float* rotations,
+                                      const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix,
+                                      const float* campos, float tan_fovx, float tan_fovy, const int* radii,
+                                      char* geom_buffer, const float* accum, float* dL_dmean2D, float* dL_dconic,
+                                      float* dL_dopacity, float* dL_dcolor, float* dL_ddepth, float* dL_dmean3D,
+                                      float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
+                                      float kernel_size, int debug, void* stream) {
+  if (!accum) { g_err = "gsr_debug_projection_backward_mip: accum is required"; return -1; }
+  if (!mip_kernel_size_ok(kernel_size)) {
+    g_err = "gsr_debug_projection_backward_mip: kernel_size must be finite and >= 0"; return -1;
+  }
+  if (P > 0 && !opacities) { g_err = "gsr_debug_projection_backward_mip: opacities are required"; return -1; }
+  BwdArgs a{};
+  a.P = P; a.D = D; a.M = M; a.W = width; a.H = height; a.radii = radii;
+  a.means3D = means3D; a.shs = shs; a.colors_precomp = colors_precomp; a.scales = scales; a.rotations = rotations;
+  a.cov3D_precomp = cov3D_precomp; a.view = viewmatrix; a.proj = projmatrix; a.campos = campos;
+  a.scale_modifier = scale_modifier; a.tan_fovx = tan_fovx; a.tan_fovy = tan_fovy;
+  a.dL_dmean2D = dL_dmean2D; a.dL_dconic = dL_dconic; a.dL_dopacity = dL_dopacity; a.dL_dcolor = dL_dcolor;
+  a.dL_ddepth = dL_ddepth; a.dL_dmean3D = dL_dmean3D; a.dL_dcov3D = dL_dcov3D; a.dL_dsh = dL_dsh;
+  a.dL_dscale = dL_dscale; a.dL_drot = dL_drot;
+  BwdHost h{};
+  h.geom_buffer = geom_buffer; h.accum = accum; h.debug = debug; h.stream = (cudaStream_t)stream;
+  h.mip = true; h.kernel_size = kernel_size; h.opacities = opacities;
   return backward_impl(a, h);
 }
 

@@ -143,6 +143,9 @@ struct BwdArgs {
   int sh_rows;  // as in FwdArgs; gradient rows leave through per-row bulk stores
 };
 void launch_preprocess_bwd(const BwdArgs& a, GeomView g, cudaStream_t st);
+// Mip-Splatting projection (2D Mip filter of width kernel_size instead of the 0.3 dilation); un-fused arguments only
+void launch_mip_preprocess_fwd(const FwdArgs& a, GeomView g, ImageView im, float kernel_size, cudaStream_t st);
+void launch_mip_preprocess_bwd(const BwdArgs& a, GeomView g, const float* opacities, float kernel_size, cudaStream_t st);
 void launch_mark_visible(int P, const float* means3D, const float* view, const float* proj,
                          unsigned char* present, cudaStream_t st);
 void launch_depth2normal(const float* depth, int W, int H, float fx, float fy, float cx, float cy, float dmin,

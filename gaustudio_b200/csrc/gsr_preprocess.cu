@@ -165,6 +165,8 @@ struct Cov2D {
   float txtz, tytz, limx, limy;
   Mat3 T, Vrk, Wm, cov;
 };
+// kMip: cov is J W Sigma W^T J^T without the 0.3 dilation (mip_filter2d adds kernel_size instead)
+template <bool kMip>
 __device__ __forceinline__ void cov2d(const V3& mean, float fx, float fy, float tan_fovx, float tan_fovy,
                                       const float* cov3D, const float* __restrict__ view, Cov2D& o) {
   o.t = xf4x3(mean, view);
@@ -186,8 +188,22 @@ __device__ __forceinline__ void cov2d(const V3& mean, float fx, float fy, float 
   o.Vrk.m[1][0] = cov3D[1]; o.Vrk.m[1][1] = cov3D[3]; o.Vrk.m[1][2] = cov3D[4];
   o.Vrk.m[2][0] = cov3D[2]; o.Vrk.m[2][1] = cov3D[4]; o.Vrk.m[2][2] = cov3D[5];
   o.cov = mmul(mmul(mtr(o.T), mtr(o.Vrk)), o.T);
-  o.cov.m[0][0] += 0.3f;
-  o.cov.m[1][1] += 0.3f;
+  if (!kMip) {
+    o.cov.m[0][0] += 0.3f;
+    o.cov.m[1][1] += 0.3f;
+  }
+}
+
+// 2D Mip filter (Mip-Splatting): the undilated cov2D (a, b, c) becomes cov' = (a + k, b, c + k), and the opacity is
+// scaled by coef = sqrt(det0 / (det1 + 1e-6) + 1e-6), det0 = max(1e-6, ac - b^2), det1 = max(1e-6, det(cov')), or 0
+// when either clamp fired.  The constants are the Mip-Splatting rasterizer's, so its checkpoints render as trained.
+__device__ __forceinline__ float mip_filter2d(Mat3& cov, float k) {
+  const float a = cov.m[0][0], b = cov.m[0][1], c = cov.m[1][1];
+  const float det0 = fmaxf(1e-6f, a * c - b * b);
+  const float det1 = fmaxf(1e-6f, (a + k) * (c + k) - b * b);
+  cov.m[0][0] = a + k;
+  cov.m[1][1] = c + k;
+  return (det0 <= 1e-6f || det1 <= 1e-6f) ? 0.f : sqrtf(det0 / (det1 + 1e-6f) + 1e-6f);
 }
 
 // Count helper: visits the binned tiles of every lane's rect.  Lanes with small rects (<= 32 tiles) loop themselves over
@@ -259,8 +275,11 @@ __device__ __forceinline__ uint32_t tile_mask_of(float px, float py, float A, fl
 
 // ---------------------------------------------------------------------------------------------
 // K1: forward.cu:155-256
+// kMip: the 2D Mip filter (mip_filter2d) replaces the 0.3 dilation and scales the opacity.  One body for both kernels,
+// inlined into each, so k_preprocess_fwd compiles to the same instructions as before the Mip variant existed.
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(PRE_THREADS, 1024 / PRE_THREADS) k_preprocess_fwd(FwdArgs a, GeomView g, ImageView im) {
+template <bool kMip>
+__device__ __forceinline__ void preprocess_fwd(FwdArgs a, GeomView g, ImageView im, float kernel_size) {
   extern __shared__ __align__(128) float sh_stage[];  // [256][3] f_dc rows, then [256][(M-1)*3] f_rest rows
   __shared__ __align__(8) unsigned long long sh_bar;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -319,7 +338,9 @@ __global__ void __launch_bounds__(PRE_THREADS, 1024 / PRE_THREADS) k_preprocess_
         for (int k = 0; k < 6; k++) g.cov3D[6 * idx + k] = c3[k];
       }
       Cov2D cc;
-      cov2d(p, a.focal_x, a.focal_y, a.tan_fovx, a.tan_fovy, c3, a.view, cc);
+      cov2d<kMip>(p, a.focal_x, a.focal_y, a.tan_fovx, a.tan_fovy, c3, a.view, cc);
+      float coef = 1.f;
+      if (kMip) coef = mip_filter2d(cc.cov, kernel_size);
       const float cx = cc.cov.m[0][0], cy = cc.cov.m[0][1], cz = cc.cov.m[1][1];
       const float det = (cx * cz - cy * cy);
       if (det != 0.0f) {
@@ -398,7 +419,8 @@ __global__ void __launch_bounds__(PRE_THREADS, 1024 / PRE_THREADS) k_preprocess_
           tiles = (uint32_t)((y1 - y0) * (x1 - x0));
           g.clamped[idx] = cl;
           float4* s = g.splat + (size_t)idx * SPLAT_F4;
-          const float opac = a.fused ? act_sigmoid(a.opacities[idx]) : a.opacities[idx];
+          float opac = a.fused ? act_sigmoid(a.opacities[idx]) : a.opacities[idx];
+          if (kMip) opac *= coef;
           // tau = 2 ln(255 o): alpha >= 1/255 needs the conic form <= tau (rectangle test of gsr_internal.cuh)
           const float4 r0 = make_float4(px, py, conA, conB), r1 = make_float4(conC, opac, p_view.z, rgb[0]);
           const float tau = 2.f * logf(255.f * opac);
@@ -432,12 +454,21 @@ __global__ void __launch_bounds__(PRE_THREADS, 1024 / PRE_THREADS) k_preprocess_
   });
   if ((bulk || rows) && threadIdx.x == 0) bar_wait0(&sh_bar);  // the copies must have landed before the CTA retires
 }
+__global__ void __launch_bounds__(PRE_THREADS, 1024 / PRE_THREADS) k_preprocess_fwd(FwdArgs a, GeomView g, ImageView im) {
+  preprocess_fwd<false>(a, g, im, 0.f);
+}
+__global__ void __launch_bounds__(PRE_THREADS, 1024 / PRE_THREADS)
+    k_mip_preprocess_fwd(FwdArgs a, GeomView g, ImageView im, float kernel_size) {
+  preprocess_fwd<true>(a, g, im, kernel_size);
+}
 
 // ---------------------------------------------------------------------------------------------
 // K6 + K7 fused: backward.cu:144-274 then 346-412 (K6 assigns dL_dmean, K7 accumulates: quirk 7)
 // ---------------------------------------------------------------------------------------------
-// 36 warps per SM (<= 56 registers): as many CTAs as the 24.6-KB SH staging block of degree 3 lets an SM hold
-__global__ void __launch_bounds__(PRE_THREADS, 1152 / PRE_THREADS) k_preprocess_bwd(BwdArgs a, GeomView g) {
+// kMip: the backward of preprocess_fwd<true>; `opacities` are the forward's input opacities (coef's gradient needs them)
+template <bool kMip>
+__device__ __forceinline__ void preprocess_bwd(BwdArgs a, GeomView g, const float* __restrict__ opacities,
+                                               float kernel_size) {
   extern __shared__ __align__(128) float sh_stage[];  // SH rows in, SH gradient rows out (in place)
   __shared__ __align__(8) unsigned long long sh_bar;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -505,7 +536,12 @@ __global__ void __launch_bounds__(PRE_THREADS, 1152 / PRE_THREADS) k_preprocess_
       c3[3] = Sg.m[1][1]; c3[4] = Sg.m[1][2]; c3[5] = Sg.m[2][2];
     }
     Cov2D cc;
-    cov2d(mean, a.focal_x, a.focal_y, a.tan_fovx, a.tan_fovy, c3, a.view, cc);
+    cov2d<kMip>(mean, a.focal_x, a.focal_y, a.tan_fovx, a.tan_fovy, c3, a.view, cc);
+    float ma = 0.f, mb = 0.f, mc = 0.f, coef = 1.f;  // kMip: the undilated cov2D and the opacity scale
+    if (kMip) {
+      ma = cc.cov.m[0][0]; mb = cc.cov.m[0][1]; mc = cc.cov.m[1][1];
+      coef = mip_filter2d(cc.cov, kernel_size);
+    }
     const float ca = cc.cov.m[0][0], cb = cc.cov.m[0][1], cd = cc.cov.m[1][1];
     const float det = ca * cd - cb * cb;  // != 0: the forward gave the Gaussian a radius
     {
@@ -529,6 +565,19 @@ __global__ void __launch_bounds__(PRE_THREADS, 1152 / PRE_THREADS) k_preprocess_
       S01 = -kreg * (h1 * ca - h0 * cb);
       S11 = -kreg * (h3 * ca - h2 * cb);
     }
+    if (kMip && coef != 0.f) {
+      // o' = o coef: dL/dcoef = dL/do' o enters dL/dcov2D through det0 = ac - b^2 and det1 = (a+k)(c+k) - b^2 (the
+      // +k is a constant; a clamp that fired left coef = 0 and passes nothing).  b fills both off-diagonal slots, so
+      // S01 takes half of d/db.
+      const float k = kernel_size;
+      const float det0 = ma * mc - mb * mb, det1 = (ma + k) * (mc + k) - mb * mb;
+      const float id1 = 1.f / (det1 + 1e-6f);
+      const float gr = dL_dopac * opacities[idx] * 0.5f / coef;  // dL/d(det0 / (det1 + 1e-6))
+      const float g0 = gr * id1, g1 = -gr * det0 * id1 * id1;    // dL/ddet0, dL/ddet1
+      S00 += g0 * mc + g1 * (mc + k);
+      S11 += g0 * ma + g1 * (ma + k);
+      S01 -= (g0 + g1) * mb;
+    }
     float A2[2][3], Vs[3][3], Wr[3][3];
 #pragma unroll
     for (int k = 0; k < 3; k++) {
@@ -540,7 +589,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 1152 / PRE_THREADS) k_preprocess_
     float SA[2][3];
 #pragma unroll
     for (int k = 0; k < 3; k++) { SA[0][k] = S00 * A2[0][k] + S01 * A2[1][k]; SA[1][k] = S01 * A2[0][k] + S11 * A2[1][k]; }
-    if (kreg != 0) {
+    if (kreg != 0 || kMip) {
       auto dV = [&](int k, int l) { return A2[0][k] * SA[0][l] + A2[1][k] * SA[1][l]; };
       dcv[0] = dV(0, 0); dcv[3] = dV(1, 1); dcv[5] = dV(2, 2);
       dcv[1] = 2.f * dV(0, 1); dcv[2] = 2.f * dV(0, 2); dcv[4] = 2.f * dV(1, 2);
@@ -632,6 +681,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 1152 / PRE_THREADS) k_preprocess_
     } else {
       dop = dL_dopac;
     }
+    if (kMip) dop *= coef;
   }
   // everything but the mean gradient is final: stored before the SH part, which only adds to dmean
   a.dL_dmean2D[3 * idx] = dm2x; a.dL_dmean2D[3 * idx + 1] = dm2y; a.dL_dmean2D[3 * idx + 2] = 0.f;
@@ -742,6 +792,14 @@ __global__ void __launch_bounds__(PRE_THREADS, 1152 / PRE_THREADS) k_preprocess_
     asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
   }
 }
+// 36 warps per SM (<= 56 registers): as many CTAs as the 24.6-KB SH staging block of degree 3 lets an SM hold
+__global__ void __launch_bounds__(PRE_THREADS, 1152 / PRE_THREADS) k_preprocess_bwd(BwdArgs a, GeomView g) {
+  preprocess_bwd<false>(a, g, nullptr, 0.f);
+}
+__global__ void __launch_bounds__(PRE_THREADS, 1152 / PRE_THREADS)
+    k_mip_preprocess_bwd(BwdArgs a, GeomView g, const float* __restrict__ opacities, float kernel_size) {
+  preprocess_bwd<true>(a, g, opacities, kernel_size);
+}
 
 // checkFrustum, rasterizer_impl.cu:54-66
 __global__ void k_mark_visible(int P, const float* __restrict__ means3D, const float* __restrict__ view,
@@ -771,6 +829,18 @@ void launch_preprocess_bwd(const BwdArgs& a, GeomView g, cudaStream_t st) {
     di.pre_bwd_smem = smem;
   }
   launch_high_priority(k_preprocess_bwd, dim3((a.P + PRE_THREADS - 1) / PRE_THREADS), dim3(PRE_THREADS), smem, st, a, g);
+}
+// The Mip entry points take the un-fused inputs only, so sh_bulk is never set and the staging block (sh_rows: 26.6 KB)
+// stays under the 48 KB that needs no opt-in.
+void launch_mip_preprocess_fwd(const FwdArgs& a, GeomView g, ImageView im, float kernel_size, cudaStream_t st) {
+  const size_t smem = a.sh_rows ? (size_t)PRE_THREADS * SH_ROW * 4 : 0;
+  launch_high_priority(k_mip_preprocess_fwd, dim3((a.P + PRE_THREADS - 1) / PRE_THREADS), dim3(PRE_THREADS), smem, st,
+                       a, g, im, kernel_size);
+}
+void launch_mip_preprocess_bwd(const BwdArgs& a, GeomView g, const float* opacities, float kernel_size, cudaStream_t st) {
+  const size_t smem = a.sh_rows ? (size_t)PRE_THREADS * SH_ROW * 4 : 0;
+  launch_high_priority(k_mip_preprocess_bwd, dim3((a.P + PRE_THREADS - 1) / PRE_THREADS), dim3(PRE_THREADS), smem, st,
+                       a, g, opacities, kernel_size);
 }
 void launch_mark_visible(int P, const float* means3D, const float* view, const float*, unsigned char* present,
                          cudaStream_t st) {

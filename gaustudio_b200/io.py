@@ -70,19 +70,25 @@ def _group(v, prefix):
 def load_ply(path, sh_degree=3, active_sh_degree=0, device="cpu"):
     """PLY -> GaussianPointCloud holding the RAW attributes (log-scale, opacity logit, un-normalised rotation),
     `_f_dc` [P,3] and `_f_rest` [P,45] exactly as `BasePointCloud.load` stores them; `active_sh_degree` starts at
-    0 like the reference model (`vanilla_sg.py:40`)."""
+    0 like the reference model (`vanilla_sg.py:40`).  A vertex element with a `filter_3D` property (a Mip-Splatting
+    checkpoint) gives a `MipPointCloud` carrying it as `filter_3D` [P,1]."""
     v = read_ply_vertices(path)
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(device)
     xyz = np.stack([v["x"], v["y"], v["z"]], axis=1)
     f_dc, f_rest = _group(v, "f_dc"), _group(v, "f_rest")
     if f_rest is None:
         f_rest = np.zeros((len(v), 3 * ((sh_degree + 1) ** 2 - 1)), np.float32)
-    return GaussianPointCloud(t(xyz), t(_group(v, "scale")), t(_group(v, "rot")), t(v["opacity"][:, None]), t(f_dc),
-                              t(f_rest), sh_degree=sh_degree, active_sh_degree=active_sh_degree)
+    args = (t(xyz), t(_group(v, "scale")), t(_group(v, "rot")), t(v["opacity"][:, None]), t(f_dc), t(f_rest))
+    if "filter_3D" in v.dtype.names:
+        from .mip import MipPointCloud
+        return MipPointCloud(*args, sh_degree=sh_degree, active_sh_degree=active_sh_degree,
+                             filter_3D=t(v["filter_3D"][:, None]))
+    return GaussianPointCloud(*args, sh_degree=sh_degree, active_sh_degree=active_sh_degree)
 
 
 def export_ply(model, path):
-    """GaussianPointCloud -> PLY in the reference's export layout (binary little-endian float32)."""
+    """GaussianPointCloud -> PLY in the reference's export layout (binary little-endian float32); a model with a
+    `filter_3D` (MipPointCloud) also writes it, last, as Mip-Splatting does."""
     n = len(model._xyz)
     flat = lambda a: a.detach().reshape(n, -1, 3).transpose(1, 2).flatten(start_dim=1).cpu().numpy()
     cols = [model._xyz.detach().cpu().numpy(), np.zeros((n, 3), np.float32), flat(model._f_dc), flat(model._f_rest),
@@ -91,6 +97,9 @@ def export_ply(model, path):
     names = ["x", "y", "z", "nx", "ny", "nz"]
     names += [f"f_dc_{i}" for i in range(cols[2].shape[1])] + [f"f_rest_{i}" for i in range(cols[3].shape[1])]
     names += ["opacity"] + [f"scale_{i}" for i in range(cols[5].shape[1])] + [f"rot_{i}" for i in range(cols[6].shape[1])]
+    if getattr(model, "filter_3D", None) is not None:
+        cols.append(model.filter_3D.detach().reshape(n, 1).cpu().numpy())
+        names.append("filter_3D")
     data = np.concatenate(cols, axis=1).astype("<f4")
     header = "ply\nformat binary_little_endian 1.0\nelement vertex %d\n" % n
     header += "".join(f"property float {nm}\n" for nm in names) + "end_header\n"

@@ -402,6 +402,56 @@ int gsr_surfel_backward(int P, int D, int M, int64_t R, const float* background,
                         const float* dL_dallmap, float* dL_dmean2D, float* dL_dopacity, float* dL_dcolor,
                         float* dL_dmean3D, float* dL_dsh, float* dL_dscale, float* dL_drot, int debug, void* stream);
 
+/* ---- Mip-Splatting: the mip_renderer (DESIGN.md, Mip-Splatting) ----
+ * gsr_forward_mip: gsr_forward with the 2D Mip filter of width kernel_size (finite, >= 0) in the projection.  Per
+ * Gaussian, with (a, b, c) = J W Sigma W^T J^T (the 2D covariance before gsr_forward's 0.3 dilation):
+ *   det0 = max(1e-6, ac - b^2), det1 = max(1e-6, (a+k)(c+k) - b^2), coef = sqrt(det0 / (det1 + 1e-6) + 1e-6), or 0
+ *   when either clamp fired;  cov' = (a+k, b, c+k) gives the conic, radius and tiles;  opacity' = opacity * coef.
+ * Everything else -- colours, depth, means2D, radii, allocators, modes, the buffers and the return value -- is
+ * gsr_forward's; gsr_debug_export reads opacity' in conic_opacity.  Only the un-fused inputs are taken.
+ * gsr_backward_mip: gsr_backward for such a forward, plus the forward's input `opacities` and the same kernel_size;
+ * dL_dopacity is w.r.t. the input opacity.  gsr_debug_projection_backward_mip: gsr_debug_projection_backward (fused = 0)
+ * for such a forward.  All three return -1 with an error text, before any work, on a bad kernel_size or NULL
+ * opacities (backward), then run the checks of the entry point they extend. */
+int64_t gsr_forward_mip(gsr_alloc_fn geometry_alloc, void* geometry_user, gsr_alloc_fn binning_alloc,
+                        void* binning_user, gsr_alloc_fn image_alloc, void* image_user, int P, int D, int M,
+                        const float* background, int width, int height, const float* means3D, const float* shs,
+                        const float* colors_precomp, const float* opacities, const float* scales,
+                        float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                        const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
+                        float tan_fovy, int prefiltered, float* out_color, float* out_depth,
+                        float* out_median_depth, float* out_opacity, int* radii, int debug, int64_t r_capacity,
+                        int64_t* r_host, float kernel_size, void* stream);
+int gsr_backward_mip(int P, int D, int M, int64_t R, const float* background, int width, int height,
+                     const float* means3D, const float* shs, const float* colors_precomp, const float* scales,
+                     float scale_modifier, const float* rotations, const float* cov3D_precomp,
+                     const float* viewmatrix, const float* projmatrix, const float* campos, float tan_fovx,
+                     float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer,
+                     const float* dL_dpix, const float* dL_dpix_depth, const float* dL_dpix_median_depth,
+                     const float* dL_dpix_final_opacity, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity,
+                     float* dL_dcolor, float* dL_ddepth, float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh,
+                     float* dL_dscale, float* dL_drot, int debug, const float* opacities, float kernel_size,
+                     void* stream);
+int gsr_debug_projection_backward_mip(int P, int D, int M, int width, int height, const float* means3D,
+                                      const float* shs, const float* colors_precomp, const float* opacities,
+                                      const float* scales, float scale_modifier, const float* rotations,
+                                      const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix,
+                                      const float* campos, float tan_fovx, float tan_fovy, const int* radii,
+                                      char* geom_buffer, const float* accum, float* dL_dmean2D, float* dL_dconic,
+                                      float* dL_dopacity, float* dL_dcolor, float* dL_ddepth, float* dL_dmean3D,
+                                      float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
+                                      float kernel_size, int debug, void* stream);
+
+/* Mip-Splatting's 3D smoothing filter (MipPointCloud.compute_3D_filter) over all cameras in one pass.
+ * cameras: DEVICE float[n_cameras*16], per camera R (9, row-major, Camera.R: p = x @ R + T), T (3), fx, fy (> 0),
+ * width, height.  Per Gaussian x: camera c sees it iff p.z > 0.2 and u = p.x/z' fx + W/2, v = p.y/z' fy + H/2
+ * (z' = max(p.z, 0.001)) lie in [-0.15 W, 1.15 W] x [-0.15 H, 1.15 H]; d = min(100000, min of p.z over those cameras);
+ * a Gaussian no camera sees gets the largest d of the seen ones; filter_3D[P] = d / max_c fx * sqrt(0.2).
+ * scratch: DEVICE uint32[3] owned by the caller; afterwards scratch[2] holds the number of seen Gaussians (when it is
+ * 0 the filter is meaningless).  No host synchronisation; the result does not depend on thread order. */
+int gsr_mip_filter3d(int P, const float* means3D, int n_cameras, const float* cameras, float* filter_3D,
+                     unsigned int* scratch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
