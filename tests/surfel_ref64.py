@@ -75,7 +75,7 @@ def project(means, scales, rots, view, proj, W, H, mod=1.0, delta=None):
         tol = 1e-6 * big / (2 * half) + 1e-5 * half
         frac = half - torch.floor(half)
         rad_amb = ok & (half > 3 * 0.707106 + 1e-6) & ((frac < tol) | (frac > 1 - tol))
-    return dict(P=P, W=W, H=H, pv=pv, Tu=Tu, Tv=Tv, Tw=Tw, nv=nv, mx=mx, my=my, d=d, radius=radius, ok=ok,
+    return dict(P=P, W=W, H=H, pv=pv, R=R, Tu=Tu, Tv=Tv, Tw=Tw, nv=nv, mx=mx, my=my, d=d, radius=radius, ok=ok,
                 rad_amb=rad_amb, depth32=pv[:, 2].detach().float())
 
 

@@ -57,11 +57,9 @@ def raw_forward(s):
 
 def _geom_records(geom, P):
     """mean2D [P,2] and packed tile rects [P,4] from the surfel geometry buffer (layout of csrc/gsr_surfel.cu)."""
-    a256 = lambda v: (v + 255) // 256 * 256
-    base = (-geom.data_ptr()) % 256
-    recA = geom[base:base + P * 48].view(torch.float32).view(P, 12)
-    off = base + a256(P * 48) + a256(P * 32)
-    rect = geom[off:off + P * 8].view(torch.int32).view(P, 2)
+    from test_gpu_surfel_f64 import geom_views
+    v = geom_views(geom, P)
+    recA, rect = v["recA"], v["rect"]
     r = torch.stack([rect[:, 0] & 0xffff, rect[:, 1] & 0xffff, (rect[:, 0] >> 16) & 0xffff, (rect[:, 1] >> 16) & 0xffff], 1)
     return recA[:, 0:2], r
 
