@@ -21,26 +21,6 @@ namespace gsr {
 namespace {
 thread_local std::string g_err;
 
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
-template <typename T> inline void take(char*& p, T*& out, size_t count) {
-  p = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(p), 256));
-  out = reinterpret_cast<T*>(p);
-  p += count * sizeof(T);
-}
-
-bool check(cudaError_t e, const char* what) {
-  if (e == cudaSuccess) return true;
-  g_err = std::string(what) + ": " + cudaGetErrorString(e);
-  return false;
-}
-// CHECK_CUDA of the reference (auxiliary.h:166-173): with debug, synchronise and surface errors per stage
-bool stage_ok(bool debug, cudaStream_t st, const char* what) {
-  if (!check(cudaGetLastError(), what)) return false;
-  if (debug && !check(cudaStreamSynchronize(st), what)) return false;
-  return true;
-}
-
 // ---- optional per-stage timing (gsr_profile_*) ----
 struct ProfRec { int stage; cudaEvent_t a, b; };
 bool g_prof_on = false;
@@ -162,10 +142,6 @@ size_t binning_bytes(long long R) {
 }
 
 namespace {
-inline char* aligned_base(char* p) { return reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(p), 256)); }
-// the projection kernels move a Gaussian's quaternion (and its gradient, and dL_dconic) as one float4
-inline bool misaligned16(const void* p) { return (reinterpret_cast<size_t>(p) & 15) != 0; }
-
 __global__ void k_init_header(ImageHeader* h, unsigned long long cap) {
   h->num_rendered = 0;
   h->num_rect = 0;
@@ -394,7 +370,7 @@ template <typename Args> void choose_sh_staging(Args& a, std::initializer_list<c
 bool first_half(const FwdArgs& a, const FwdHost& h, GeomView g, ImageView im, unsigned long long cap) {
   const int T = a.gx * a.gy;
   if (!check(cudaMemsetAsync(im.tile_count, 0, sizeof(uint32_t) * T * SUBBINS, h.stream), "memset tile_count")) return false;
-  launch_high_priority(k_init_header, dim3(1), dim3(1), 0, h.stream, im.hdr, cap);
+  launch_init_header(im.hdr, cap, h.stream);
   {
     Prof pf(kPreprocessFwd, h.stream);
     if (h.mip) launch_mip_preprocess_fwd(a, g, im, h.kernel_size, h.stream);
@@ -510,6 +486,10 @@ int backward_impl(BwdArgs& a, const BwdHost& h) {
 }  // namespace
 
 void set_last_error(const char* msg) { g_err = msg; }
+
+void launch_init_header(ImageHeader* hdr, unsigned long long cap, cudaStream_t st) {
+  launch_high_priority(k_init_header, dim3(1), dim3(1), 0, st, hdr, cap);
+}
 
 namespace {
 bool mip_kernel_size_ok(float k) { return std::isfinite(k) && k >= 0.f; }

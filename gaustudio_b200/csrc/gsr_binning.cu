@@ -315,7 +315,7 @@ __global__ void __launch_bounds__(SCATTER_THREADS) k_scatter(int P, int gx, int 
         if (slot[k] < limit) b.ents[slot[k]] = key;
     }
   }
-  // a splat covering many tiles is walked by the whole warp (see for_each_tile in gsr_preprocess.cu)
+  // a splat covering many tiles is walked by the whole warp (see for_each_tile in gsr_internal.cuh)
   unsigned big = __ballot_sync(FULL, n > kBig);
   while (big) {
     const int src = __ffs(big) - 1;

@@ -6,6 +6,8 @@
 #include <stdint.h>
 #include <stddef.h>
 
+#include <string>
+
 namespace gsr {
 
 constexpr int TILE_X = 16;  // observable behaviour of the reference (config.h:16-17; SURVEY.md §8b)
@@ -116,6 +118,8 @@ struct FwdArgs {
 };
 
 // ---- launch wrappers (each enqueues on `st`) ----
+// zeroes the header's counters and sets the binning capacity the scatter / sort / render kernels may use
+void launch_init_header(ImageHeader* hdr, unsigned long long cap, cudaStream_t st);
 void launch_preprocess_fwd(const FwdArgs& a, GeomView g, ImageView im, cudaStream_t st);
 void launch_tile_scan(ImageView im, int T, cudaStream_t st);
 int set_tile_order(int mode);  // gsr_set_tile_order
@@ -171,6 +175,41 @@ __device__ __forceinline__ uint2 pack_rect(int xmin, int ymin, int xmax, int yma
 }
 __device__ __forceinline__ void unpack_rect(uint2 r, int& xmin, int& ymin, int& xmax, int& ymax) {
   xmin = r.x & 0xffff; xmax = r.x >> 16; ymin = r.y & 0xffff; ymax = r.y >> 16;
+}
+
+// auxiliary.h:46-56
+__device__ __forceinline__ void tile_rect(float px, float py, int max_radius, int gx, int gy, int& x0, int& y0,
+                                          int& x1, int& y1) {
+  x0 = min(gx, max((int)0, (int)((px - max_radius) / TILE_X)));
+  y0 = min(gy, max((int)0, (int)((py - max_radius) / TILE_Y)));
+  x1 = min(gx, max((int)0, (int)((px + max_radius + TILE_X - 1) / TILE_X)));
+  y1 = min(gy, max((int)0, (int)((py + max_radius + TILE_Y - 1) / TILE_Y)));
+}
+
+// Count helper: visits the binned tiles of every lane's rect.  Lanes with small rects (<= 32 tiles) loop themselves over
+// the set bits of their tile mask; large rects (a splat covering much of the screen) are walked in full by the
+// whole warp so one thread never serialises thousands of atomics (the reference's duplicateWithKeys does,
+// rasterizer_impl.cu:98-108).
+constexpr int kBigRect = 32;
+template <typename F>
+__device__ __forceinline__ void for_each_tile(int x0, int y0, int x1, int y1, uint32_t mask, int gx, F f) {
+  const int w = x1 - x0, n = w * (y1 - y0);
+  const unsigned lane = threadIdx.x & 31;
+  if (n > 0 && n <= kBigRect) {
+    while (mask) {
+      const int i = __ffs(mask) - 1;
+      mask &= mask - 1;
+      f((y0 + i / w) * gx + x0 + i % w, lane);
+    }
+  }
+  unsigned big = __ballot_sync(0xffffffffu, n > kBigRect);
+  while (big) {
+    const int src = __ffs(big) - 1;
+    big &= big - 1;
+    const int bx0 = __shfl_sync(0xffffffffu, x0, src), by0 = __shfl_sync(0xffffffffu, y0, src);
+    const int bw = __shfl_sync(0xffffffffu, w, src), bn = __shfl_sync(0xffffffffu, n, src);
+    for (int i = lane; i < bn; i += 32) f((by0 + i / bw) * gx + bx0 + i % bw, (unsigned)src);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -273,5 +312,29 @@ int launch_adam(int n_groups, const gsr_adam_group* groups, double beta1, double
 
 // the text gsr_last_error() returns next (gsr_api.cu keeps it); for entry points defined in other sources
 void set_last_error(const char* msg);
+
+// ---- host helpers of the entry points ----
+inline size_t align256(size_t v) { return (v + 255) / 256 * 256; }
+// carves `count` elements from p at its next 256-byte boundary and advances p past them
+template <typename T> inline void take(char*& p, T*& out, size_t count) {
+  p = reinterpret_cast<char*>(align256(reinterpret_cast<size_t>(p)));
+  out = reinterpret_cast<T*>(p);
+  p += count * sizeof(T);
+}
+inline char* aligned_base(char* p) { return reinterpret_cast<char*>(align256(reinterpret_cast<size_t>(p))); }
+// the projection kernels move a Gaussian's quaternion (and its gradient, and dL_dconic) as one float4
+inline bool misaligned16(const void* p) { return (reinterpret_cast<size_t>(p) & 15) != 0; }
+
+inline bool check(cudaError_t e, const char* what) {
+  if (e == cudaSuccess) return true;
+  set_last_error((std::string(what) + ": " + cudaGetErrorString(e)).c_str());
+  return false;
+}
+// CHECK_CUDA of the reference (auxiliary.h:166-173): with debug, synchronise and surface errors per stage
+inline bool stage_ok(bool debug, cudaStream_t st, const char* what) {
+  if (!check(cudaGetLastError(), what)) return false;
+  if (debug && !check(cudaStreamSynchronize(st), what)) return false;
+  return true;
+}
 
 }  // namespace gsr

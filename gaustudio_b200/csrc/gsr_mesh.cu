@@ -48,7 +48,6 @@ struct TsdfView {
   unsigned long long tmask;        // T - 1
 };
 
-inline size_t align256(size_t v) { return (v + 255) / 256 * 256; }
 // The table holds up to 4x the brick pool (at least 64 Ki keys), so a pool that runs out still counts the distinct
 // bricks the scene needs and the error can name that number; within the pool the load factor stays <= 1/4.
 inline unsigned long long table_size(long long cap) {

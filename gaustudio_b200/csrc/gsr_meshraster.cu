@@ -60,8 +60,6 @@ struct RasterCtx {
   long long* ends;           // [F] inclusive scan of cnt
 };
 
-inline size_t align256(size_t v) { return (v + 255) / 256 * 256; }
-
 struct RasterLayout {
   size_t keys, hdr, vrec, cnt, ends, tmp, tmp_bytes, total;
 };

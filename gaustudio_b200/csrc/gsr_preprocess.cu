@@ -125,15 +125,6 @@ __device__ __forceinline__ float4 xf4x4(const V3& p, const float* __restrict__ m
 // auxiliary.h:41-44: the 1.0 / 0.5 literals make this a double-precision expression
 __device__ __forceinline__ float ndc2pix(float v, int S) { return ((v + 1.0) * S - 1.0) * 0.5; }
 
-// auxiliary.h:46-56
-__device__ __forceinline__ void tile_rect(float px, float py, int max_radius, int gx, int gy, int& x0, int& y0,
-                                          int& x1, int& y1) {
-  x0 = min(gx, max((int)0, (int)((px - max_radius) / TILE_X)));
-  y0 = min(gy, max((int)0, (int)((py - max_radius) / TILE_Y)));
-  x1 = min(gx, max((int)0, (int)((px + max_radius + TILE_X - 1) / TILE_X)));
-  y1 = min(gy, max((int)0, (int)((py + max_radius + TILE_Y - 1) / TILE_Y)));
-}
-
 struct Rot { Mat3 R; };
 // rotation from the un-normalised quaternion (r,x,y,z) exactly as forward.cu:127-139 (quirk 2)
 __device__ __forceinline__ Mat3 quat_mat(float r, float x, float y, float z) {
@@ -204,32 +195,6 @@ __device__ __forceinline__ float mip_filter2d(Mat3& cov, float k) {
   cov.m[0][0] = a + k;
   cov.m[1][1] = c + k;
   return (det0 <= 1e-6f || det1 <= 1e-6f) ? 0.f : sqrtf(det0 / (det1 + 1e-6f) + 1e-6f);
-}
-
-// Count helper: visits the binned tiles of every lane's rect.  Lanes with small rects (<= 32 tiles) loop themselves over
-// the set bits of their tile mask; large rects (a splat covering much of the screen) are walked in full by the
-// whole warp so one thread never serialises thousands of atomics (the reference's duplicateWithKeys does,
-// rasterizer_impl.cu:98-108).
-constexpr int kBigRect = 32;
-template <typename F>
-__device__ __forceinline__ void for_each_tile(int x0, int y0, int x1, int y1, uint32_t mask, int gx, F f) {
-  const int w = x1 - x0, n = w * (y1 - y0);
-  const unsigned lane = threadIdx.x & 31;
-  if (n > 0 && n <= kBigRect) {
-    while (mask) {
-      const int i = __ffs(mask) - 1;
-      mask &= mask - 1;
-      f((y0 + i / w) * gx + x0 + i % w, lane);
-    }
-  }
-  unsigned big = __ballot_sync(0xffffffffu, n > kBigRect);
-  while (big) {
-    const int src = __ffs(big) - 1;
-    big &= big - 1;
-    const int bx0 = __shfl_sync(0xffffffffu, x0, src), by0 = __shfl_sync(0xffffffffu, y0, src);
-    const int bw = __shfl_sync(0xffffffffu, w, src), bn = __shfl_sync(0xffffffffu, n, src);
-    for (int i = lane; i < bn; i += 32) f((by0 + i / bw) * gx + bx0 + i % bw, (unsigned)src);
-  }
 }
 
 // Which tiles of a Gaussian's rect [x0,x1) x [y0,y1) (<= 32 tiles) can it contribute to at all?  Bit i (row-major in the

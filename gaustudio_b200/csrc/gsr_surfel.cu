@@ -41,14 +41,6 @@ struct SurfImage {
   uint32_t* med_c;  // [H*W] 1 + position in the tile list of the median splat; 0: none
 };
 
-inline size_t align256(size_t v) { return (v + 255) / 256 * 256; }
-template <typename T> inline void take(char*& p, T*& out, size_t count) {
-  p = reinterpret_cast<char*>(align256(reinterpret_cast<size_t>(p)));
-  out = reinterpret_cast<T*>(p);
-  p += count * sizeof(T);
-}
-inline char* aligned_base(char* p) { return reinterpret_cast<char*>(align256(reinterpret_cast<size_t>(p))); }
-
 SurfGeom carve_sgeom(char* base, int P) {
   SurfGeom g;
   char* p = base;
@@ -164,14 +156,6 @@ __device__ __forceinline__ bool surfel_project(int idx, const float* __restrict_
   return isfinite(s.mx) && isfinite(s.my) && s.radius < 1e7f;
 }
 
-// the reference's getRect on 16x16 tiles
-__device__ __forceinline__ void surfel_rect(float px, float py, int r, int gx, int gy, int& x0, int& y0, int& x1, int& y1) {
-  x0 = min(gx, max((int)0, (int)((px - r) / TILE_X)));
-  y0 = min(gy, max((int)0, (int)((py - r) / TILE_Y)));
-  x1 = min(gx, max((int)0, (int)((px + r + TILE_X - 1) / TILE_X)));
-  y1 = min(gy, max((int)0, (int)((py + r + TILE_Y - 1) / TILE_Y)));
-}
-
 // SH basis (the 3DGS path's constants and ordering)
 __device__ __forceinline__ int sh_basis(int D, F3 d, float w[16], F3 gw[16]) {
   constexpr float C0 = 0.28209479177387814f, C1 = 0.4886025119029199f;
@@ -232,15 +216,16 @@ __device__ __forceinline__ float dist_m(float z) { return kFar / (kFar - kNear) 
 __device__ __forceinline__ float dist_dm(float z) { return kFar / (kFar - kNear) * kNear / (z * z); }
 
 // ---- projection forward --------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(SURF_THREADS) k_surfel_project(SurfArgs a, SurfGeom g, ImageView im) {
+// 10 CTAs per SM: keeps the kernel at 48 registers (the shared tile walk alone would let ptxas take 50, and 9 CTAs)
+__global__ void __launch_bounds__(SURF_THREADS, 10) k_surfel_project(SurfArgs a, SurfGeom g, ImageView im) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
-  uint32_t tiles = 0;
+  uint32_t tiles = 0, tmask = 0;
   if (idx < a.P) {
     int radius_i = 0;
     SurfProj s;
     if (surfel_project(idx, a.means3D, a.scales, a.rotations, a.mod, a.view, a.proj, a.W, a.H, s)) {
-      surfel_rect(s.mx, s.my, (int)s.radius, a.gx, a.gy, x0, y0, x1, y1);
+      tile_rect(s.mx, s.my, (int)s.radius, a.gx, a.gy, x0, y0, x1, y1);
       if ((x1 - x0) * (y1 - y0) != 0) {
         float rgb[3];
         unsigned char cl = 0;
@@ -276,25 +261,17 @@ __global__ void __launch_bounds__(SURF_THREADS) k_surfel_project(SurfArgs a, Sur
     g.radii[idx] = radius_i;
     if (a.radii_out) a.radii_out[idx] = radius_i;
     g.rect[idx] = pack_rect(x0, y0, x1, y1);
-    g.tile_mask[idx] = tiles >= 32 ? 0xffffffffu : ((1u << tiles) - 1u);  // no exact tile culling: the whole rect
+    tmask = tiles >= 32 ? 0xffffffffu : ((1u << tiles) - 1u);  // no exact tile culling: the whole rect
+    g.tile_mask[idx] = tmask;
   }
   // num_rendered = sum of the rect areas: one atomic per warp
   const unsigned wsum = __reduce_add_sync(0xffffffffu, tiles);
   if ((threadIdx.x & 31) == 0 && wsum) atomicAdd(&im.hdr->num_rect, (unsigned long long)wsum);
-  // sub-binned tile histogram: small rects by their own lane, large ones by the whole warp
-  const int T = a.gx * a.gy, w = x1 - x0, n = (int)tiles;
-  const unsigned lane = threadIdx.x & 31;
-  if (n > 0 && n <= 32)
-    for (int i = 0; i < n; i++) atomicAdd(&im.tile_count[subbin_of(idx) * T + (y0 + i / w) * a.gx + x0 + i % w], 1u);
-  unsigned big = __ballot_sync(0xffffffffu, n > 32);
-  while (big) {
-    const int src = __ffs(big) - 1;
-    big &= big - 1;
-    const int bx0 = __shfl_sync(0xffffffffu, x0, src), by0 = __shfl_sync(0xffffffffu, y0, src);
-    const int bw = __shfl_sync(0xffffffffu, w, src), bn = __shfl_sync(0xffffffffu, n, src);
-    const int sidx = __shfl_sync(0xffffffffu, idx, src);
-    for (int i = lane; i < bn; i += 32) atomicAdd(&im.tile_count[subbin_of(sidx) * T + (by0 + i / bw) * a.gx + bx0 + i % bw], 1u);
-  }
+  // sub-binned tile histogram
+  const int T = a.gx * a.gy, warp_base = idx - (int)(threadIdx.x & 31);
+  for_each_tile(x0, y0, x1, y1, tmask, a.gx, [&](int tile, unsigned src) {
+    atomicAdd(&im.tile_count[subbin_of(warp_base + (int)src) * T + tile], 1u);
+  });
 }
 
 // ---- compositing forward: one CTA per 16x16 tile, records staged in batches of 256 ---------------------------------
@@ -589,27 +566,6 @@ __global__ void __launch_bounds__(SURF_THREADS) k_surfel_project_bwd(SurfBwdArgs
   }
 }
 
-__global__ void k_surfel_init_header(ImageHeader* h) {
-  h->num_rendered = 0;
-  h->num_rect = 0;
-  h->capacity = ~0ull;
-  h->overflow = 0;
-  h->num_big = 0;
-  h->ticket[0] = 0;
-  h->ticket[1] = 0;
-}
-
-bool fail(const char* what, cudaError_t e) {
-  set_last_error((std::string(what) + ": " + cudaGetErrorString(e)).c_str());
-  return false;
-}
-bool stage_ok(int debug, cudaStream_t st, const char* what) {
-  cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess && debug) e = cudaStreamSynchronize(st);
-  return e == cudaSuccess || fail(what, e);
-}
-inline bool misaligned16(const void* p) { return (reinterpret_cast<size_t>(p) & 15) != 0; }
-
 const char* surfel_args_error(int P, int D, int M, int W, int H, const float* means3D, const float* shs,
                               const float* colors, const float* scales, const float* rotations, const float* view,
                               const float* proj, const float* campos, const float* bg) {
@@ -659,9 +615,8 @@ int64_t gsr_surfel_forward(gsr_alloc_fn geometry_alloc, void* geometry_user, gsr
   if (!gbuf || !ibuf) { set_last_error("gsr_surfel_forward: scratch allocation failed"); return -1; }
   const SurfGeom g = carve_sgeom(aligned_base(gbuf), P);
   const SurfImage si = carve_simage(aligned_base(ibuf), W, H);
-  cudaError_t e = cudaMemsetAsync(si.im.tile_count, 0, sizeof(uint32_t) * T * SUBBINS, st);
-  if (e != cudaSuccess) { fail("memset tile_count", e); return -1; }
-  k_surfel_init_header<<<1, 1, 0, st>>>(si.im.hdr);
+  if (!check(cudaMemsetAsync(si.im.tile_count, 0, sizeof(uint32_t) * T * SUBBINS, st), "memset tile_count")) return -1;
+  launch_init_header(si.im.hdr, ~0ull, st);
   if (P > 0) {
     SurfArgs a{P, D, M, W, H, gx, gy, means3D, shs, colors_precomp, opacities, scales, rotations, viewmatrix,
                projmatrix, cam_pos, scale_modifier, radii};
@@ -672,9 +627,9 @@ int64_t gsr_surfel_forward(gsr_alloc_fn geometry_alloc, void* geometry_user, gsr
   if (!stage_ok(debug, st, "tile_scan")) return -1;
   // the one blocking read: the instance count sizes the binning buffer
   unsigned long long counts[2] = {0, 0};  // {binned, rect-sum}: adjacent header fields (equal here: no tile culling)
-  e = cudaMemcpyAsync(counts, &si.im.hdr->num_rendered, sizeof(counts), cudaMemcpyDeviceToHost, st);
+  cudaError_t e = cudaMemcpyAsync(counts, &si.im.hdr->num_rendered, sizeof(counts), cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) { fail("read R", e); return -1; }
+  if (!check(e, "read R")) return -1;
   const long long binned = (long long)counts[0];
   char* bbuf = binning_alloc(binning_user, binning_bytes(binned));
   if (!bbuf) { set_last_error("gsr_surfel_forward: binning allocation failed"); return -1; }
@@ -717,8 +672,7 @@ int gsr_surfel_backward(int P, int D, int M, int64_t R, const float* background,
   const cudaStream_t st = (cudaStream_t)stream;
   const int W = width, H = height, gx = (W + TILE_X - 1) / TILE_X, gy = (H + TILE_Y - 1) / TILE_Y;
   const SurfGeom g = carve_sgeom(aligned_base(geom_buffer), P);
-  cudaError_t e = cudaMemsetAsync(g.grad, 0, sizeof(float) * SURF_GRAD * (size_t)P, st);
-  if (e != cudaSuccess) { fail("memset grad", e); return -1; }
+  if (!check(cudaMemsetAsync(g.grad, 0, sizeof(float) * SURF_GRAD * (size_t)P, st), "memset grad")) return -1;
   if (R > 0) {
     const SurfImage si = carve_simage(aligned_base(image_buffer), W, H);
     const BinView b = carve_binning(aligned_base(binning_buffer), R);

@@ -17,6 +17,23 @@ def cpu_deep_copy_tuple(input_tuple):
     return tuple(item.cpu().clone() if isinstance(item, torch.Tensor) else item for item in input_tuple)
 
 
+def call_with_snapshot(fn, args, debug, path, message):
+    """fn(*args).  With `debug`, a CPU copy of `args` taken before the call is saved to `path` if the call raises, and
+    `message` is printed before the exception propagates (__init__.py:83-90)."""
+    if not debug:
+        return fn(*args)
+    cpu_args = cpu_deep_copy_tuple(args)  # copy before they can be corrupted
+    try:
+        return fn(*args)
+    except Exception as ex:
+        torch.save(cpu_args, path)
+        print(message)
+        raise ex
+
+
+FW_MESSAGE = "\nAn error occured in forward. Please forward snapshot_fw.dump for debugging."
+
+
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         raster_settings):
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
@@ -24,28 +41,30 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales,
 
 
 class _RasterizeGaussians(torch.autograd.Function):
+    """Settings with a `kernel_size` field (gaustudio_b200.mip_rasterizer) select the Mip-Splatting projection, whose
+    backward also needs the input opacities."""
+
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 raster_settings):
         rs = raster_settings
+        mip = hasattr(rs, "kernel_size")
         args = (rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
                 rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, sh,
                 rs.sh_degree, rs.campos, rs.prefiltered, rs.debug)
-        if rs.debug:
-            cpu_args = cpu_deep_copy_tuple(args)  # copy before they can be corrupted (__init__.py:83-90)
-            try:
-                out = _C.rasterize_gaussians(*args)
-            except Exception as ex:
-                torch.save(cpu_args, "snapshot_fw.dump")
-                print("\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
-                raise ex
+        if mip:
+            out = call_with_snapshot(_C.rasterize_gaussians_mip, args + (rs.kernel_size,), rs.debug,
+                                     "snapshot_fw.dump", FW_MESSAGE)
         else:
-            out = _C.rasterize_gaussians(*args)
+            out = call_with_snapshot(_C.rasterize_gaussians, args, rs.debug, "snapshot_fw.dump", FW_MESSAGE)
         num_rendered, color, depth, median_depth, final_opacity, radii, geomBuffer, binningBuffer, imgBuffer = out
         ctx.raster_settings = rs
         ctx.num_rendered = num_rendered
-        ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
-                              binningBuffer, imgBuffer)
+        saved = (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer,
+                 imgBuffer)
+        if mip:
+            saved += (opacities,)
+        ctx.save_for_backward(*saved)
         ctx.mark_non_differentiable(radii)
         return color, radii, depth, median_depth, final_opacity
 
@@ -53,21 +72,17 @@ class _RasterizeGaussians(torch.autograd.Function):
     def backward(ctx, grad_out_color, grad_radii, grad_depth, grad_median_depth, grad_final_opacity):
         rs = ctx.raster_settings
         (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer,
-         imgBuffer) = ctx.saved_tensors
-        args = (rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
-                rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color, grad_depth, grad_median_depth,
-                grad_final_opacity, sh, rs.sh_degree, rs.campos, geomBuffer, ctx.num_rendered, binningBuffer,
-                imgBuffer, rs.debug)
-        if rs.debug:
-            cpu_args = cpu_deep_copy_tuple(args)
-            try:
-                out = _C.rasterize_gaussians_backward(*args)
-            except Exception as ex:
-                torch.save(cpu_args, "snapshot_bw.dump")
-                print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
-                raise ex
+         imgBuffer, *mip_opacities) = ctx.saved_tensors
+        tail = (scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx,
+                rs.tanfovy, grad_out_color, grad_depth, grad_median_depth, grad_final_opacity, sh, rs.sh_degree,
+                rs.campos, geomBuffer, ctx.num_rendered, binningBuffer, imgBuffer, rs.debug)
+        message = "\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n"
+        if mip_opacities:
+            args = (rs.bg, means3D, radii, colors_precomp, *mip_opacities, *tail, rs.kernel_size)
+            out = call_with_snapshot(_C.rasterize_gaussians_mip_backward, args, rs.debug, "snapshot_bw.dump", message)
         else:
-            out = _C.rasterize_gaussians_backward(*args)
+            args = (rs.bg, means3D, radii, colors_precomp, *tail)
+            out = call_with_snapshot(_C.rasterize_gaussians_backward, args, rs.debug, "snapshot_bw.dump", message)
         (grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_cov3Ds_precomp, grad_sh, grad_scales,
          grad_rotations) = out
         # order of the reference (__init__.py:146-156)
@@ -127,7 +142,17 @@ class GaussianRasterizationSettings(NamedTuple):
     debug: bool
 
 
+def check_exactly_one_of(shs, colors_precomp, scales, rotations, cov3D_precomp):
+    if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
+        raise Exception('Please provide excatly one of either SHs or precomputed colors!')
+    if ((scales is None or rotations is None) and cov3D_precomp is None) or \
+            ((scales is not None or rotations is not None) and cov3D_precomp is not None):
+        raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
+
+
 class GaussianRasterizer(nn.Module):
+    _function = _RasterizeGaussians  # the autograd Function `forward` applies
+
     def __init__(self, raster_settings):
         super().__init__()
         self.raster_settings = raster_settings
@@ -139,12 +164,7 @@ class GaussianRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3D_precomp=None):
-        rs = self.raster_settings
-        if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
-            raise Exception('Please provide excatly one of either SHs or precomputed colors!')
-        if ((scales is None or rotations is None) and cov3D_precomp is None) or \
-                ((scales is not None or rotations is not None) and cov3D_precomp is not None):
-            raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
+        check_exactly_one_of(shs, colors_precomp, scales, rotations, cov3D_precomp)
         empty = torch.Tensor([])
         if shs is None:
             shs = empty
@@ -156,5 +176,5 @@ class GaussianRasterizer(nn.Module):
             rotations = empty
         if cov3D_precomp is None:
             cov3D_precomp = empty
-        return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                   rs)
+        return self._function.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
+                                    cov3D_precomp, self.raster_settings)

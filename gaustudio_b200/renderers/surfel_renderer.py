@@ -4,68 +4,16 @@
 import torch
 
 from . import register
-from .base import settings_for
-from .vanilla_renderer import eval_sh
+from .base import BaseRenderer
+from ..surfel_rasterizer import GaussianRasterizer
 
 
 @register('surfel_renderer')
-class SurfelRenderer:
-    default_conf = {
-        'kernel_size': 0.,
-        'scaling_modifier': 1.,
-        'white_background': False,
-        'convert_SHs_python': False,
-        'compute_cov3D_python': False,
-        'debug': False,
-    }
-
-    def __init__(self, config) -> None:
-        self.config = {**self.default_conf, **config}
-        self.kernel_size = self.config['kernel_size']
-        self.scaling_modifier = self.config['scaling_modifier']
-        self.white_background = self.config['white_background']
-        # kept on the CPU like the 3DGS renderer; the binding caches a device copy
-        self.bg_color = torch.tensor([1, 1, 1] if self.white_background else [0, 0, 0], dtype=torch.float32)
-        self.convert_SHs_python = self.config['convert_SHs_python']
-        self.compute_cov3D_python = self.config['compute_cov3D_python']
-        self.debug = self.config['debug']
-
-    def get_gaussians_properties(self, viewpoint_camera, gaussian_model):
-        xyz = gaussian_model.get_attribute("xyz")
-        opacity = gaussian_model.get_attribute("opacity")
-        scales = rotations = cov3D_precomp = None
-        if self.compute_cov3D_python:
-            cov3D_precomp = gaussian_model.get_covariance(self.scaling_modifier)
-        else:
-            scales = gaussian_model.get_attribute("scale")
-            rotations = gaussian_model.get_attribute("rot")
-        shs = colors_precomp = None
-        if self.convert_SHs_python:
-            feats = gaussian_model.get_features
-            shs_view = feats.transpose(1, 2).view(-1, 3, (gaussian_model.max_sh_degree + 1) ** 2)
-            dir_pp = xyz - viewpoint_camera.camera_center.repeat(feats.shape[0], 1)
-            sh2rgb = eval_sh(gaussian_model.active_sh_degree, shs_view, dir_pp / dir_pp.norm(dim=1, keepdim=True))
-            colors_precomp = torch.clamp_min(sh2rgb + 0.5, 0.0)
-        else:
-            shs = gaussian_model.get_features
-        return xyz, shs, colors_precomp, opacity, scales, rotations, cov3D_precomp
+class SurfelRenderer(BaseRenderer):
+    rasterizer = GaussianRasterizer
 
     def render(self, viewpoint_camera, gaussian_model):
-        from ..surfel_rasterizer import GaussianRasterizer
-        xyz, shs, colors_precomp, opacity, scales, rotations, cov3D_precomp = \
-            self.get_gaussians_properties(viewpoint_camera, gaussian_model)
-        # a zero tensor in the graph: autograd hands back the screen-space statistic through it
-        screenspace = torch.zeros_like(xyz, requires_grad=True) + 0
-        try:
-            screenspace.retain_grad()
-        except Exception:
-            pass
-        degree = gaussian_model.active_sh_degree if shs is not None else 1
-        rs = settings_for(viewpoint_camera, bg=self.bg_color, scale_modifier=self.scaling_modifier, sh_degree=degree,
-                          debug=self.debug)
-        image, radii, allmap = GaussianRasterizer(raster_settings=rs)(
-            means3D=xyz, means2D=screenspace, shs=shs, colors_precomp=colors_precomp, opacities=opacity,
-            scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp)
+        (image, radii, allmap), screenspace = self.rasterize(viewpoint_camera, gaussian_model)
         alpha = allmap[1:2]
         normal = (allmap[2:5].permute(1, 2, 0) @ viewpoint_camera.world_view_transform[:3, :3].T).permute(2, 0, 1)
         median = torch.nan_to_num(allmap[5:6], 0, 0)

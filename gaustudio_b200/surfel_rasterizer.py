@@ -11,28 +11,15 @@ surfel rasterizer).
 from typing import NamedTuple
 
 import torch
-import torch.nn as nn
 
-from . import _C
-from .rasterizer import cpu_deep_copy_tuple
+from . import _C, rasterizer
+from .rasterizer import FW_MESSAGE, call_with_snapshot, check_exactly_one_of, cpu_deep_copy_tuple  # noqa: F401
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         raster_settings):
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                      cov3Ds_precomp, raster_settings)
-
-
-def _call(fn, args, debug, name, what):
-    if not debug:
-        return fn(*args)
-    cpu_args = cpu_deep_copy_tuple(args)  # copy before they can be corrupted
-    try:
-        return fn(*args)
-    except Exception as ex:
-        torch.save(cpu_args, name)
-        print(f"\nAn error occured in {what}. Please forward {name} for debugging.")
-        raise ex
 
 
 class _RasterizeGaussians(torch.autograd.Function):
@@ -47,8 +34,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         args = (rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, rs.viewmatrix,
                 rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, sh, rs.sh_degree, rs.campos,
                 rs.prefiltered, rs.debug)
-        num_rendered, color, radii, allmap, geomBuffer, binningBuffer, imgBuffer = _call(
-            _C.rasterize_surfels, args, rs.debug, "snapshot_fw.dump", "forward")
+        num_rendered, color, radii, allmap, geomBuffer, binningBuffer, imgBuffer = call_with_snapshot(
+            _C.rasterize_surfels, args, rs.debug, "snapshot_fw.dump", FW_MESSAGE)
         ctx.raster_settings = rs
         ctx.num_rendered = num_rendered
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, radii, sh, geomBuffer, binningBuffer,
@@ -64,7 +51,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                 rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color, grad_allmap, sh, rs.sh_degree, rs.campos,
                 geomBuffer, ctx.num_rendered, binningBuffer, imgBuffer, rs.debug)
         (grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_sh, grad_scales,
-         grad_rotations) = _call(_C.rasterize_surfels_backward, args, rs.debug, "snapshot_bw.dump", "backward")
+         grad_rotations) = call_with_snapshot(_C.rasterize_surfels_backward, args, rs.debug, "snapshot_bw.dump",
+                                              "\nAn error occured in backward. Please forward snapshot_bw.dump for debugging.")
         return (grad_means3D, grad_means2D, grad_sh, grad_colors_precomp, grad_opacities, grad_scales, grad_rotations,
                 None, None)
 
@@ -84,29 +72,12 @@ class GaussianRasterizationSettings(NamedTuple):
     debug: bool
 
 
-class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings):
-        super().__init__()
-        self.raster_settings = raster_settings
-
-    def markVisible(self, positions):
-        with torch.no_grad():
-            rs = self.raster_settings
-            return _C.mark_visible(positions, rs.viewmatrix, rs.projmatrix)
+class GaussianRasterizer(rasterizer.GaussianRasterizer):
+    _function = _RasterizeGaussians
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3D_precomp=None):
-        rs = self.raster_settings
-        if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
-            raise Exception('Please provide excatly one of either SHs or precomputed colors!')
-        if ((scales is None or rotations is None) and cov3D_precomp is None) or \
-                ((scales is not None or rotations is not None) and cov3D_precomp is not None):
-            raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
         if cov3D_precomp is not None:
+            check_exactly_one_of(shs, colors_precomp, scales, rotations, cov3D_precomp)
             raise NotImplementedError("surfel rasterizer: precomputed splat transforms (cov3D_precomp) are not supported")
-        empty = torch.Tensor([])
-        if shs is None:
-            shs = empty
-        if colors_precomp is None:
-            colors_precomp = empty
-        return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, empty, rs)
+        return super().forward(means3D, means2D, opacities, shs, colors_precomp, scales, rotations)

@@ -3,7 +3,7 @@ and the forward's per-pixel maps, each with a magnitude that bounds what float32
 
 Inputs are the forward's own per-Gaussian records (mean2D, Tu, Tv, Tw, opacity, the float32 view depth that is the sort
 key, n_view, rgb) and the integer radii, promoted to float64, so that the projection's rounding does not enter.  Per-tile
-lists are built here: the kernel's surfel_rect in float32 on the record's mean2D and the integer radius (every tile of
+lists are built here: the kernel's tile_rect in float32 on the record's mean2D and the integer radius (every tile of
 the rect, no exact tile culling), sorted by (float32 depth, index).  The GPU's binned list is not used.
 
 A pixel (x, y) (integer coordinates) walks its tile's list front to back with the contract's rules (DESIGN.md §3, surfel
@@ -99,7 +99,7 @@ def unpack_records(recA, recB):
 
 
 def surfel_rects(mean2D, radii, W, H):
-    """The kernel's surfel_rect in float32: x0 = (px - r) / 16, x1 = (px + r + 16 - 1) / 16 (left to right),
+    """The kernel's tile_rect in float32: x0 = (px - r) / 16, x1 = (px + r + 16 - 1) / 16 (left to right),
     truncated toward zero and clamped to the grid -> int64 [P,4] (x0, y0, x1, y1) and the grid size."""
     gx, gy = (W + TILE - 1) // TILE, (H + TILE - 1) // TILE
     m = np.asarray(torch.as_tensor(mean2D).detach().cpu().numpy(), dtype=np.float32).reshape(-1, 2)
