@@ -465,6 +465,89 @@ def mip_filter3d(means3D, cameras):
     return out
 
 
+# ---- Scaffold-GS: gsr_scaffold_visible / _count / _decode / _decode_backward (include/gsr.h) ----------------------------
+def scaffold_visible(means3D, scales, rotations, cov3D_precomp, scale_modifier, viewmatrix, projmatrix, tan_fovx,
+                     tan_fovy, image_height, image_width, kernel_size):
+    """radii [N] (int32) of Gaussians at `means3D` under the Mip projection of width kernel_size: bit-identical to the
+    radii rasterize_gaussians_mip gives them.  scales [N,3] + rotations [N,4], or cov3D_precomp [N,6]."""
+    if not means3D.is_cuda:
+        raise RuntimeError("gaustudio_b200 runs on CUDA (sm_90a) only; means3D must be a CUDA tensor")
+    dev = means3D.device
+    N = means3D.size(0)
+    radii = torch.empty(N, dtype=torch.int32, device=dev)
+    means3D = _f32(means3D, dev, "means3D"); scales = _f32(scales, dev, "scales")
+    rotations = _f32_rot(rotations, dev, "rotations"); cov3D_precomp = _f32(cov3D_precomp, dev, "cov3D_precomp")
+    viewmatrix = _f32(viewmatrix, dev, "viewmatrix"); projmatrix = _f32(projmatrix, dev, "projmatrix")
+    with _on_device(dev):
+        rc = _lib.lib().gsr_scaffold_visible(N, _ptr(means3D), _ptr(scales), _ptr(rotations), _ptr(cov3D_precomp),
+                                             float(scale_modifier), _ptr(viewmatrix), _ptr(projmatrix),
+                                             int(image_width), int(image_height), float(tan_fovx), float(tan_fovy),
+                                             _check_kernel_size(kernel_size), _ptr(radii),
+                                             torch.cuda.current_stream(dev).cuda_stream)
+    if rc < 0:
+        raise RuntimeError("gsr_scaffold_visible failed: " + _lib.last_error())
+    return radii
+
+
+def scaffold_count(opacity):
+    """opacity [Nv,k] (the opacity MLP's output) -> (base [Nv+1] int32, M): exclusive prefix of the offsets kept per
+    visible anchor (opacity > 0) and their total, read back to the host (one synchronisation)."""
+    dev = opacity.device
+    Nv, k = opacity.shape
+    opacity = _f32(opacity, dev, "opacity")
+    buf = torch.empty(Nv + 1 + (Nv + 1023) // 1024, dtype=torch.int32, device=dev)
+    with _on_device(dev):
+        rc = _lib.lib().gsr_scaffold_count(Nv, k, _ptr(opacity), _ptr(buf), _ptr(buf[Nv + 1:]),
+                                           torch.cuda.current_stream(dev).cuda_stream)
+    if rc < 0:
+        raise RuntimeError("gsr_scaffold_count failed: " + _lib.last_error())
+    base = buf[:Nv + 1]
+    return base, int(base[Nv])
+
+
+def scaffold_decode(vis, base, M, anchor, offset, scaling, opacity, color, cov):
+    """The kept neural Gaussians, rows anchor-major and offset-minor: (xyz [M,3], rgb [M,3], opacity [M,1],
+    scales [M,3], rotations [M,4]).  vis [Nv] int64; anchor [N,3], offset [N,k,3], scaling [N,6] full-size; opacity
+    [Nv,k], color [Nv,3k], cov [Nv,7k]; base, M from scaffold_count."""
+    dev = anchor.device
+    Nv, k = opacity.shape
+    e = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+    out = (e(M, 3), e(M, 3), e(M, 1), e(M, 3), e(M, 4))
+    ins = [_f32(t, dev, n) for t, n in ((anchor, "anchor"), (offset, "offset"), (scaling, "scaling"),
+                                        (opacity, "opacity"), (color, "color"), (cov, "cov"))]
+    vis = vis.contiguous()
+    if M > 0:
+        with _on_device(dev):
+            rc = _lib.lib().gsr_scaffold_decode(Nv, k, _ptr(vis), _ptr(base), *[_ptr(t) for t in ins],
+                                                *[_ptr(t) for t in out], torch.cuda.current_stream(dev).cuda_stream)
+        if rc < 0:
+            raise RuntimeError("gsr_scaffold_decode failed: " + _lib.last_error())
+    return out
+
+
+def scaffold_decode_backward(vis, base, M, offset, scaling, opacity, cov, grads):
+    """Backward of scaffold_decode.  grads: the upstream gradients of its five outputs (None: zero).
+    -> (d_anchor [N,3], d_offset [N,k,3], d_scaling [N,6], d_opacity [Nv,k], d_color [Nv,3k], d_cov [Nv,7k])."""
+    dev = offset.device
+    N, k = offset.shape[0], offset.shape[1]
+    Nv = opacity.shape[0]
+    e = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+    d_anchor, d_offset, d_scaling = e(N, 3), e(N, k, 3), e(N, 6)
+    d_op, d_col, d_cov = e(Nv, k), e(Nv, 3 * k), e(Nv, 7 * k)
+    offset, scaling = _f32(offset, dev, "offset"), _f32(scaling, dev, "scaling")
+    opacity, cov = _f32(opacity, dev, "opacity"), _f32(cov, dev, "cov")
+    g = [torch.zeros(M, w, dtype=torch.float32, device=dev) if t is None else _f32(t, dev, "grad")
+         for t, w in zip(grads, (3, 3, 1, 3, 4))]
+    with _on_device(dev):
+        rc = _lib.lib().gsr_scaffold_decode_backward(
+            N, Nv, k, _ptr(vis.contiguous()), _ptr(base), _ptr(offset), _ptr(scaling), _ptr(opacity), _ptr(cov),
+            *[_ptr(t) for t in g], _ptr(d_op), _ptr(d_col), _ptr(d_cov), _ptr(d_anchor), _ptr(d_offset),
+            _ptr(d_scaling), torch.cuda.current_stream(dev).cuda_stream)
+    if rc < 0:
+        raise RuntimeError("gsr_scaffold_decode_backward failed: " + _lib.last_error())
+    return d_anchor, d_offset, d_scaling, d_op, d_col, d_cov
+
+
 def mark_visible(means3D, viewmatrix, projmatrix):
     L = _lib.lib()
     dev = means3D.device

@@ -68,6 +68,11 @@ SIGNATURES = {
     "gsr_debug_projection_backward_mip": (_I, [_I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _F, _P, _P, _P, _P, _P, _F, _F,
                                                _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _F, _I, _P]),
     "gsr_mip_filter3d": (_I, [_I, _P, _I, _P, _P, _P, _P]),
+    "gsr_scaffold_visible": (_I, [_I, _P, _P, _P, _P, _F, _P, _P, _I, _I, _F, _F, _F, _P, _P]),
+    "gsr_scaffold_count": (_I, [_I, _I, _P, _P, _P, _P]),
+    "gsr_scaffold_decode": (_I, [_I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "gsr_scaffold_decode_backward": (_I, [_I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                          _P, _P]),
 }
 
 _lib = None

@@ -152,6 +152,15 @@ void launch_mip_preprocess_fwd(const FwdArgs& a, GeomView g, ImageView im, float
 void launch_mip_preprocess_bwd(const BwdArgs& a, GeomView g, const float* opacities, float kernel_size, cudaStream_t st);
 void launch_mark_visible(int P, const float* means3D, const float* view, const float* proj,
                          unsigned char* present, cudaStream_t st);
+// Scaffold-GS anchor visibility (gsr_scaffold_visible, gsr_scaffold.cu): radii[P] of the Mip projection of width
+// kernel_size, un-fused scales [P,3] + rotations [P,4] or cov3D_precomp [P,6]
+struct ScaffoldVisArgs {
+  int P, W, H;
+  const float *means3D, *scales, *rotations, *cov3D_precomp, *view, *proj;
+  float scale_modifier, tan_fovx, tan_fovy, kernel_size;
+  int* radii;
+};
+void launch_scaffold_visible(const ScaffoldVisArgs& a, cudaStream_t st);
 void launch_depth2normal(const float* depth, int W, int H, float fx, float fy, float cx, float cy, float dmin,
                          float dmax, const float* rot, float* out, cudaStream_t st);
 void launch_depth2point(const float* depth, int W, int H, float fx, float fy, float cx, float cy, const float* c2w,

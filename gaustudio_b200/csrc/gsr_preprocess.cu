@@ -775,6 +775,55 @@ __global__ void k_mark_visible(int P, const float* __restrict__ means3D, const f
   present[idx] = xf4x3(p, view).z > 0.2f;
 }
 
+// Scaffold-GS anchor visibility (gsr_scaffold_visible): the radius preprocess_fwd<true> gives a Gaussian with the same
+// mean, covariance and camera, and nothing else.  Same near-plane test, cov2d<true> + mip_filter2d, eigenvalue floor,
+// ceil and tile_rect area test; the radius does not depend on the opacity, so none is read.  The radius lines are
+// written here rather than moved into a helper shared with preprocess_fwd, whose instructions must stay as they are.
+__global__ void __launch_bounds__(PRE_THREADS)
+    k_scaffold_visible(ScaffoldVisArgs a, float focal_x, float focal_y, int gx, int gy) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= a.P) return;
+  int radius_i = 0;
+  const V3 p = {a.means3D[3 * idx], a.means3D[3 * idx + 1], a.means3D[3 * idx + 2]};
+  const V3 p_view = xf4x3(p, a.view);
+  if (p_view.z > 0.2f) {
+    const float4 p_hom = xf4x4(p, a.proj);
+    const float p_w = 1.0f / (p_hom.w + 0.0000001f);
+    const float ppx = p_hom.x * p_w, ppy = p_hom.y * p_w;
+    float c3[6];
+    if (a.cov3D_precomp != nullptr) {
+#pragma unroll
+      for (int k = 0; k < 6; k++) c3[k] = a.cov3D_precomp[6 * idx + k];
+    } else {
+      const float mod = a.scale_modifier;
+      const float s0 = a.scales[3 * idx], s1 = a.scales[3 * idx + 1], s2 = a.scales[3 * idx + 2];
+      const float4 q = reinterpret_cast<const float4*>(a.rotations)[idx];
+      const Mat3 S = scale_mat(mod * s0, mod * s1, mod * s2);
+      const Mat3 R = quat_mat(q.x, q.y, q.z, q.w);
+      const Mat3 Mm = mmul(S, R);
+      const Mat3 Sg = mmul(mtr(Mm), Mm);
+      c3[0] = Sg.m[0][0]; c3[1] = Sg.m[0][1]; c3[2] = Sg.m[0][2];
+      c3[3] = Sg.m[1][1]; c3[4] = Sg.m[1][2]; c3[5] = Sg.m[2][2];
+    }
+    Cov2D cc;
+    cov2d<true>(p, focal_x, focal_y, a.tan_fovx, a.tan_fovy, c3, a.view, cc);
+    mip_filter2d(cc.cov, a.kernel_size);
+    const float cx = cc.cov.m[0][0], cy = cc.cov.m[0][1], cz = cc.cov.m[1][1];
+    const float det = (cx * cz - cy * cy);
+    if (det != 0.0f) {
+      const float mid = 0.5f * (cx + cz);
+      const float lambda1 = mid + sqrt(max(0.1f, mid * mid - det));
+      const float lambda2 = mid - sqrt(max(0.1f, mid * mid - det));
+      const float my_radius = ceil(3.f * sqrt(max(lambda1, lambda2)));
+      const float px = ndc2pix(ppx, a.W), py = ndc2pix(ppy, a.H);
+      int x0, y0, x1, y1;
+      tile_rect(px, py, (int)my_radius, gx, gy, x0, y0, x1, y1);
+      if ((x1 - x0) * (y1 - y0) != 0) radius_i = (int)my_radius;
+    }
+  }
+  a.radii[idx] = radius_i;
+}
+
 }  // namespace
 
 void launch_preprocess_fwd(const FwdArgs& a, GeomView g, ImageView im, cudaStream_t st) {
@@ -810,6 +859,12 @@ void launch_mip_preprocess_bwd(const BwdArgs& a, GeomView g, const float* opacit
 void launch_mark_visible(int P, const float* means3D, const float* view, const float*, unsigned char* present,
                          cudaStream_t st) {
   k_mark_visible<<<(P + 255) / 256, 256, 0, st>>>(P, means3D, view, present);
+}
+// focal lengths and tile grid from the host expressions of forward_impl (gsr_api.cu), so they are the same floats
+void launch_scaffold_visible(const ScaffoldVisArgs& a, cudaStream_t st) {
+  const float focal_y = a.H / (2.0f * a.tan_fovy), focal_x = a.W / (2.0f * a.tan_fovx);
+  const int gx = (a.W + TILE_X - 1) / TILE_X, gy = (a.H + TILE_Y - 1) / TILE_Y;
+  k_scaffold_visible<<<(a.P + PRE_THREADS - 1) / PRE_THREADS, PRE_THREADS, 0, st>>>(a, focal_x, focal_y, gx, gy);
 }
 
 }  // namespace gsr

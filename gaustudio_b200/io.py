@@ -108,6 +108,82 @@ def export_ply(model, path):
         f.write(data.tobytes())
 
 
+_SCAFFOLD_MLPS = (("mlp_opacity", "opacity_mlp.pt"), ("mlp_cov", "cov_mlp.pt"), ("mlp_color", "color_mlp.pt"),
+                  ("mlp_feature_bank", "feature_bank_mlp.pt"))
+
+
+def _plain_mlp(path, device):
+    """A TorchScript MLP (Linear, ReLU, Linear[, activation]) as a plain nn.Sequential with its `0.*` / `2.*` weights;
+    the activation is the module the traced one ends with."""
+    from torch import nn
+    ts = torch.jit.load(path, map_location="cpu")
+    sd = ts.state_dict()
+    w0, w2 = sd["0.weight"], sd["2.weight"]
+    layers = [nn.Linear(w0.shape[1], w0.shape[0]), nn.ReLU(True), nn.Linear(w2.shape[1], w2.shape[0])]
+    tail = [getattr(ts, n).original_name for n, _ in ts.named_children()][3:]
+    acts = {"Tanh": nn.Tanh(), "Sigmoid": nn.Sigmoid(), "Softmax": nn.Softmax(dim=1)}
+    for name in tail:
+        if name not in acts:
+            raise ValueError(f"{path}: unsupported layer {name} after the second Linear")
+        layers.append(acts[name])
+    mlp = nn.Sequential(*layers)
+    mlp.load_state_dict({k: v for k, v in sd.items() if k.split(".")[0] in ("0", "2")})
+    return mlp.to(device)
+
+
+def load_scaffold(ply_path, mlp_dir=None, device="cpu"):
+    """A Scaffold-GS checkpoint -> ScaffoldPointCloud.  The PLY's vertex element holds x y z nx ny nz f_offset_*
+    f_anchor_feat_* opacity scale_0..5 rot_0..3, the offsets channel-major (f_offset_{c*k+j} is channel c of offset j);
+    `mlp_dir` (default: the PLY's directory) holds the TorchScript MLPs opacity_mlp.pt, cov_mlp.pt, color_mlp.pt and
+    optionally feature_bank_mlp.pt, whose weights are copied into plain modules."""
+    import os
+    from .scaffold import ScaffoldPointCloud
+    v = read_ply_vertices(ply_path)
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(device)
+    n = len(v)
+    offset = _group(v, "f_offset")
+    if offset is None or offset.shape[1] % 3:
+        raise ValueError(f"{ply_path}: no f_offset_* columns, or not a multiple of 3")
+    offset = offset.reshape(n, 3, -1).transpose(0, 2, 1)
+    mlp_dir = os.path.dirname(os.path.abspath(ply_path)) if mlp_dir is None else mlp_dir
+    mlps = {}
+    for attr, fname in _SCAFFOLD_MLPS:
+        p = os.path.join(mlp_dir, fname)
+        if os.path.exists(p):
+            mlps[attr] = _plain_mlp(p, device)
+        elif attr != "mlp_feature_bank":
+            raise FileNotFoundError(p)
+    return ScaffoldPointCloud(t(np.stack([v["x"], v["y"], v["z"]], axis=1)), t(offset), t(_group(v, "f_anchor_feat")),
+                              t(v["opacity"][:, None]), t(_group(v, "scale")), t(_group(v, "rot")), **mlps)
+
+
+def export_scaffold(model, ply_path):
+    """ScaffoldPointCloud -> the layout load_scaffold reads: the PLY (binary little-endian float32) and, next to it, the
+    MLPs traced to TorchScript on the CPU."""
+    import copy
+    import os
+    n = model.num_points
+    cols = [model._anchor, torch.zeros(n, 3), model._offset.transpose(1, 2).reshape(n, -1), model._anchor_feat,
+            model._opacity.reshape(n, 1), model._scale, model._rot]
+    cols = [c.detach().cpu().numpy().astype("<f4") for c in cols]
+    names = ["x", "y", "z", "nx", "ny", "nz"] + [f"f_offset_{i}" for i in range(cols[2].shape[1])]
+    names += [f"f_anchor_feat_{i}" for i in range(cols[3].shape[1])] + ["opacity"]
+    names += [f"scale_{i}" for i in range(6)] + [f"rot_{i}" for i in range(4)]
+    header = "ply\nformat binary_little_endian 1.0\nelement vertex %d\n" % n
+    header += "".join(f"property float {nm}\n" for nm in names) + "end_header\n"
+    with open(ply_path, "wb") as f:
+        f.write(header.encode("ascii"))
+        f.write(np.concatenate(cols, axis=1).astype("<f4").tobytes())
+    out_dir = os.path.dirname(os.path.abspath(ply_path))
+    for attr, fname in _SCAFFOLD_MLPS:
+        mlp = getattr(model, attr)
+        if mlp is None:
+            continue
+        m = copy.deepcopy(mlp).cpu().eval()
+        x = torch.rand(1, m[0].in_features)
+        torch.jit.trace(m, x).save(os.path.join(out_dir, fname))
+
+
 def export_points_ply(path, xyz, rgb=None, normals=None):
     """Surface point cloud (the `fused.ply` of gaustudio/scripts/extract_pcd.py:339-352, written there through
     open3d's `write_point_cloud`): binary little-endian, double x y z [nx ny nz] + uchar red green blue, the property

@@ -153,7 +153,8 @@ def extract_mesh(renderer, pcd, cameras, voxel_size=0.01, sdf_trunc=0.04, min_we
     the final opacity is >= 0.5, lift it to world points and fuse it, then run marching cubes.  The reference's
     striding (`cameras[::3]`) and downscaling are the caller's choice, as in `extract.extract_pcd`.
     -> (vertices [V,3] float32, faces [F,3] int64), CUDA."""
-    volume = TSDFVolume(voxel_size, sdf_trunc, capacity_bricks=capacity_bricks, device=pcd._xyz.device)
+    device = pcd._anchor.device if hasattr(pcd, "_anchor") else pcd._xyz.device  # Scaffold-GS anchors, or Gaussians
+    volume = TSDFVolume(voxel_size, sdf_trunc, capacity_bricks=capacity_bricks, device=device)
     for camera in cameras:
         with torch.no_grad():
             pkg = renderer.render(camera, pcd)

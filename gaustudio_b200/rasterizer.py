@@ -162,6 +162,21 @@ class GaussianRasterizer(nn.Module):
             rs = self.raster_settings
             return _C.mark_visible(positions, rs.viewmatrix, rs.projmatrix)
 
+    def visible_filter(self, means3D, scales=None, rotations=None, cov3D_precomp=None):
+        """Radii [N] the Mip projection of the settings' `kernel_size` gives Gaussians at `means3D`, with nothing
+        rendered: the Mip-Splatting fork's method, which Scaffold-GS uses to find the anchors in view.  Needs settings
+        with a `kernel_size` (gaustudio_b200.mip_rasterizer); the radii equal those the forward would return."""
+        rs = self.raster_settings
+        if not hasattr(rs, "kernel_size"):
+            raise TypeError("visible_filter needs rasterization settings with a kernel_size (gaustudio_b200.mip_rasterizer)")
+        if ((scales is None or rotations is None) and cov3D_precomp is None) or \
+                ((scales is not None or rotations is not None) and cov3D_precomp is not None):
+            raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
+        with torch.no_grad():
+            return _C.scaffold_visible(means3D, scales, rotations, cov3D_precomp, rs.scale_modifier, rs.viewmatrix,
+                                       rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width,
+                                       rs.kernel_size)
+
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3D_precomp=None):
         check_exactly_one_of(shs, colors_precomp, scales, rotations, cov3D_precomp)

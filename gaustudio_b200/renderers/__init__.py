@@ -35,3 +35,4 @@ def make(config):
 from . import vanilla_renderer  # noqa: E402,F401  (the only renderer on the hot path; SURVEY.md §2.1)
 from . import surfel_renderer  # noqa: E402,F401  (2DGS: configs/2dgs.yaml)
 from . import mip_renderer  # noqa: E402,F401  (Mip-Splatting)
+from . import scaffold_renderer  # noqa: E402,F401  (Scaffold-GS)

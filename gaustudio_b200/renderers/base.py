@@ -113,10 +113,11 @@ class BaseRenderer:
         return settings_for(viewpoint_camera, bg=self.bg_color, scale_modifier=self.scaling_modifier,
                             sh_degree=sh_degree, debug=self.debug)
 
-    def rasterize(self, viewpoint_camera, gaussian_model):
-        """The rasterizer's outputs for one view, and the screen-space tensor its 2-D mean gradients arrive in."""
+    def rasterize(self, viewpoint_camera, gaussian_model, props=None):
+        """The rasterizer's outputs for one view, and the screen-space tensor its 2-D mean gradients arrive in.
+        props: the 7-tuple of get_gaussians_properties when the caller has it already."""
         xyz, shs, colors_precomp, opacity, scales, rotations, cov3D_precomp = \
-            self.get_gaussians_properties(viewpoint_camera, gaussian_model)
+            props if props is not None else self.get_gaussians_properties(viewpoint_camera, gaussian_model)
         # a zero tensor in the graph: autograd hands back the 2-D (screen-space) mean gradients through it
         screenspace = torch.zeros_like(xyz, requires_grad=True) + 0
         try:

@@ -452,6 +452,43 @@ int gsr_debug_projection_backward_mip(int P, int D, int M, int width, int height
 int gsr_mip_filter3d(int P, const float* means3D, int n_cameras, const float* cameras, float* filter_3D,
                      unsigned int* scratch, void* stream);
 
+/* ---- Scaffold-GS: the scaffold_renderer (DESIGN.md §7d) ----
+ * gsr_scaffold_visible: radii[N] (int32) of N Gaussians at the anchors, with activated scales[N,3] (times
+ * scale_modifier) and rotations[N,4] (16-byte aligned), or cov3D_precomp[N,6], under the Mip projection of width
+ * kernel_size (finite, >= 0).  Bit-identical to the radii gsr_forward_mip writes for the same means, scales,
+ * rotations and camera (the radius does not depend on the opacity).  No host synchronisation. */
+int gsr_scaffold_visible(int N, const float* means3D, const float* scales, const float* rotations,
+                         const float* cov3D_precomp, float scale_modifier, const float* viewmatrix,
+                         const float* projmatrix, int width, int height, float tan_fovx, float tan_fovy,
+                         float kernel_size, int* radii, void* stream);
+
+/* Neural-Gaussian decoding of Nv visible anchors with k = 1..32 offsets each.  opacity[Nv,k] (the opacity MLP's
+ * output); offset j of visible anchor i is kept iff opacity[i,j] > 0.
+ * gsr_scaffold_count: base[Nv+1] (int32) = exclusive prefix of the kept counts, base[Nv] = M; scratch: DEVICE
+ * int32[(Nv + 1023) / 1024].  No host synchronisation.
+ * gsr_scaffold_decode: kept rows in anchor-major, offset-minor order (row base[i] + rank of j among i's kept offsets).
+ * vis[Nv] (int64): anchor index of visible anchor i; anchor[N,3], offset[N,k,3], scaling[N,6] (activated) are
+ * full-size; color[Nv,3k] and cov[Nv,7k] are the colour and covariance MLPs' outputs.  For v = vis[i],
+ * S = scaling[v], c = color[i,3j..], s = cov[i,7j..]:
+ *   xyz[M,3] = anchor[v] + offset[v,j] * S[0:3]   rgb[M,3] = c   out_opacity[M] = opacity[i,j]
+ *   scales[M,3] = S[3:6] * sigmoid(s[0:3])        rotations[M,4] = s[3:7] / max(|s[3:7]|, 1e-12) (16-byte aligned)
+ * each product and sum rounded on its own.
+ * gsr_scaffold_decode_backward: with the upstream gradients of the five outputs ([M,...], read only where M > 0),
+ * writes dL_dopacity_mlp[Nv,k], dL_dcolor[Nv,3k], dL_dcov[Nv,7k] (zero for dropped offsets) and the full-size
+ * dL_danchor[N,3], dL_doffset[N,k,3], dL_dscaling[N,6] (zero for anchors that are not visible and for dropped offsets).
+ * One thread per visible anchor sums its offsets in order: no atomics, the same bits on every run.
+ * All three return -1 with an error text, before any work, on k outside 1..32, Nv < 0 (or Nv > N), a product of
+ * the sizes beyond int32, NULL required pointers or misaligned rotations. */
+int gsr_scaffold_count(int Nv, int k, const float* opacity, int* base, int* scratch, void* stream);
+int gsr_scaffold_decode(int Nv, int k, const int64_t* vis, const int* base, const float* anchor, const float* offset,
+                        const float* scaling, const float* opacity, const float* color, const float* cov, float* xyz,
+                        float* rgb, float* out_opacity, float* scales, float* rotations, void* stream);
+int gsr_scaffold_decode_backward(int N, int Nv, int k, const int64_t* vis, const int* base, const float* offset,
+                                 const float* scaling, const float* opacity, const float* cov, const float* dL_dxyz,
+                                 const float* dL_drgb, const float* dL_dopacity, const float* dL_dscales,
+                                 const float* dL_drotations, float* dL_dopacity_mlp, float* dL_dcolor, float* dL_dcov,
+                                 float* dL_danchor, float* dL_doffset, float* dL_dscaling, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
