@@ -100,7 +100,9 @@ class Compositing:
     """The geometry-only half of the reference for one forward: per-tile contributors, transmittances, flags and error
     gains.  `sums(upstream)` then gives the ten sums for any upstream images."""
 
-    def __init__(self, means2D, conic_opacity, rgb, depths, radii, W, H, bg, rect_dtype=np.float32):
+    def __init__(self, means2D, conic_opacity, rgb, depths, radii, W, H, bg, rect_dtype=np.float32, lists=None):
+        """lists: per-tile Gaussian lists to composite instead of the ones built here from the tile rectangles (a
+        forward's own sorted list, when the question is what the compositing made of THAT list)."""
         self.W, self.H = int(W), int(H)
         self.m2 = _t64(means2D).reshape(-1, 2)
         self.co = _t64(conic_opacity).reshape(-1, 4)
@@ -108,7 +110,10 @@ class Compositing:
         self.depth = _t64(depths).reshape(-1)
         self.bg = _t64(bg).reshape(3)
         self.P = self.m2.shape[0]
-        lists, self.gx, self.gy = tile_lists(means2D, radii, depths, W, H, rect_dtype)
+        self.gx, self.gy = (self.W + TILE - 1) // TILE, (self.H + TILE - 1) // TILE
+        if lists is None:
+            lists, _, _ = tile_lists(means2D, radii, depths, W, H, rect_dtype)
+        assert len(lists) == self.gx * self.gy
         self.tiles = []
         HW = self.W * self.H
         self.flag = torch.zeros(HW, dtype=torch.bool)         # alpha, power or stop decision ambiguous
@@ -118,6 +123,7 @@ class Compositing:
         self.ended = torch.zeros(HW, dtype=torch.bool)        # the pixel ended on T < 1e-4
         self.final_T = torch.ones(HW, dtype=F64)
         self.median = torch.full((HW,), -1, dtype=torch.int64)  # Gaussian at which T crosses 0.5, -1: none
+        self.last = torch.zeros(HW, dtype=torch.int64)  # 1 + list position of the last contributor (forward.cu's n_contrib)
         self.flag_kinds = {k: torch.zeros(HW, dtype=torch.bool) for k in ("alpha", "power", "stop", "median")}
         for t, ids in enumerate(lists):
             if ids:
@@ -174,6 +180,7 @@ class Compositing:
         self.flag_median[pid] = f_med
         self.covered[pid] = contrib.any(1)
         self.n_contrib[pid] = contrib.sum(1)
+        self.last[pid] = (contrib * (pos + 1)).max(1).values
         self.ended[pid] = kstop < n
         self.final_T[pid] = T_final
         has_med = med.any(1)

@@ -273,6 +273,16 @@ def test_fused_path_with_mostly_culled_ctas_matches_unfused():
         # the forward is deterministic: say which of the two renders does not reproduce, and where
         again = render_both()
         stable = {f: all(np.array_equal(x, y) for x, y in zip(imgs[f], again[f])) for f in (False, True)}
+        # `again` took the speculative form (the shape has a hint now) while the first un-fused render took the plain
+        # blocking form: re-render through the plain form too, so that like is compared with like
+        from gaustudio_b200 import _C
+        prev = _C.set_speculation(False)
+        try:
+            plain = render_both()
+        finally:
+            _C.set_speculation(prev)
+        first_vs_plain = {f: all(np.array_equal(x, y) for x, y in zip(imgs[f], plain[f])) for f in (False, True)}
+        plain_vs_spec = {f: all(np.array_equal(x, y) for x, y in zip(plain[f], again[f])) for f in (False, True)}
         d = np.abs(imgs[True][0] - imgs[False][0]).max(axis=0)
         pad = np.zeros((192, 240), np.float32); pad[:180] = d
         per_tile = pad.reshape(12, 16, 15, 16).max(axis=(1, 3))
@@ -281,7 +291,9 @@ def test_fused_path_with_mostly_culled_ctas_matches_unfused():
         moved = {f: [float(np.abs(x - y).max()) for x, y in zip(imgs[f], again[f])] for f in (False, True)}
         raise AssertionError(f"{ex}; re-render reproduces: unfused {stable[False]}, fused {stable[True]}; tiles over 1e-4: "
                              f"{int((per_tile > 1e-4).sum())}/180, worst {[(int(t), float(per_tile.ravel()[t])) for t in worst]}; "
-                             f"max |first - re-render| of (colour, depth, opacity): unfused {moved[False]}, fused {moved[True]}")
+                             f"max |first - re-render| of (colour, depth, opacity): unfused {moved[False]}, fused {moved[True]}; "
+                             f"first == plain-path re-render: unfused {first_vs_plain[False]}, fused {first_vs_plain[True]}; "
+                             f"plain-path == speculative re-render: unfused {plain_vs_spec[False]}, fused {plain_vs_spec[True]}")
 
 
 def test_views_on_concurrent_streams_match_sequential():
