@@ -1,6 +1,6 @@
-// C ABI of libgsr_b200 (include/gsr.h): buffer carving, stage orchestration, error reporting.
-// Orchestration restates CudaRasterizer::Rasterizer::{forward,backward,markVisible}
-// ($RAST/cuda_rasterizer/rasterizer_impl.cu:141-153, 198-343, 347-452) on top of the H100 kernels.
+// C ABI of the rasterizer (include/gsr.h): buffer carving, stage orchestration, depth maps, state export, and the
+// error text of every entry point.  Orchestration restates CudaRasterizer::Rasterizer::{forward,backward}
+// ($RAST/cuda_rasterizer/rasterizer_impl.cu:198-343, 347-452) on top of the H100 kernels.
 #include "../../include/gsr.h"
 #include "gsr_internal.cuh"
 #include <cmath>
@@ -20,6 +20,7 @@ namespace gsr {
 
 namespace {
 thread_local std::string g_err;
+void set_last_error(const char* msg) { g_err = msg; }
 
 // ---- optional per-stage timing (gsr_profile_*) ----
 struct ProfRec { int stage; cudaEvent_t a, b; };
@@ -285,29 +286,6 @@ __global__ void k_export_image(int N, int T, ImageView im, uint32_t* ranges, uin
 }
 }  // namespace
 
-void launch_depth2normal(const float* depth, int W, int H, float fx, float fy, float cx, float cy, float dmin,
-                         float dmax, const float* rot, float* out, cudaStream_t st) {
-  dim3 blk(32, 8), grd((W + 31) / 32, (H + 7) / 8);
-  // K^-1 entries computed on the host in float like torch.inverse of the float32 intrinsics
-  launch_high_priority(k_depth2normal, grd, blk, 0, st, depth, W, H, 1.0f / fx, 1.0f / fy, -cx / fx, -cy / fy, dmin, dmax, rot, out);
-}
-
-void launch_depth2point(const float* depth, int W, int H, float fx, float fy, float cx, float cy, const float* c2w,
-                        float* out, cudaStream_t st) {
-  dim3 blk(32, 8), grd((W + 31) / 32, (H + 7) / 8);
-  k_depth2point<<<grd, blk, 0, st>>>(depth, W, H, 1.0f / fx, 1.0f / fy, -cx / fx, -cy / fy, c2w, out);
-}
-
-void launch_debug_export(int P, int W, int H, long long R, GeomView g, BinView b, ImageView im,
-                         uint32_t* point_list, uint32_t* ranges, uint32_t* n_contrib, float* final_T,
-                         float* means2D, float* conic_opacity, float* depths, float* rgb, float* cov3D,
-                         uint32_t* tiles_touched, unsigned char* clamped, cudaStream_t st) {
-  if (P > 0) k_export_geom<<<(P + 255) / 256, 256, 0, st>>>(P, g, means2D, conic_opacity, depths, rgb, cov3D, tiles_touched, clamped);
-  if (R > 0 && point_list) k_export_list<<<(unsigned)((R + 255) / 256), 256, 0, st>>>(R, im.hdr, b, point_list);
-  const int N = W * H, T = ((W + TILE_X - 1) / TILE_X) * ((H + TILE_Y - 1) / TILE_Y);
-  k_export_image<<<(max(N, T) + 255) / 256, 256, 0, st>>>(N, T, im, ranges, n_contrib, final_T);
-}
-
 namespace {
 // what a forward takes besides the kernels' arguments (FwdArgs)
 struct FwdHost {
@@ -383,7 +361,7 @@ bool first_half(const FwdArgs& a, const FwdHost& h, GeomView g, ImageView im, un
 // second half of the forward for a given binning capacity: scatter, per-tile sort, compositing
 bool second_half(const FwdArgs& a, const FwdHost& h, GeomView g, ImageView im, long long cap) {
   char* bbuf = h.binning_alloc(h.binning_user, binning_bytes(cap));
-  if (!bbuf) { g_err = "gsr_forward: binning allocation failed"; return false; }
+  if (!bbuf) { set_last_error("gsr_forward: binning allocation failed"); return false; }
   BinView b = carve_binning(aligned_base(bbuf), cap);
   if (cap > 0) {
     { Prof pf(kScatter, h.stream); launch_scatter(a.P, a.gx, a.gx * a.gy, g, im, b, h.stream); }
@@ -423,10 +401,10 @@ int64_t forward_speculative(const FwdArgs& a, const FwdHost& h, GeomView g, Imag
 // reference's num_rendered = sum of the rect areas (what the API returns in exact mode).
 int64_t forward_impl(FwdArgs& a, const FwdHost& h) {
   a.gx = (a.W + TILE_X - 1) / TILE_X; a.gy = (a.H + TILE_Y - 1) / TILE_Y;
-  if (const char* e = forward_error(a)) { g_err = e; return -1; }
+  if (const char* e = forward_error(a)) { set_last_error(e); return -1; }
   char* gbuf = h.geometry_alloc(h.geometry_user, geom_bytes(a.P));
   char* ibuf = h.image_alloc(h.image_user, image_bytes(a.W, a.H));
-  if (!gbuf || !ibuf) { g_err = "gsr_forward: scratch allocation failed"; return -1; }
+  if (!gbuf || !ibuf) return fail("gsr_forward", "scratch allocation failed");
   GeomView g = carve_geom(aligned_base(gbuf), a.P);
   ImageView im = carve_image(aligned_base(ibuf), a.W, a.H);
   a.focal_y = a.H / (2.0f * a.tan_fovy);  // rasterizer_impl.cu:225-226
@@ -456,7 +434,7 @@ int64_t forward_impl(FwdArgs& a, const FwdHost& h) {
 
 int backward_impl(BwdArgs& a, const BwdHost& h) {
   if (a.P <= 0) return 0;
-  if (const char* e = backward_error(a, h)) { g_err = e; return -1; }
+  if (const char* e = backward_error(a, h)) { set_last_error(e); return -1; }
   GeomView g = carve_geom(aligned_base(h.geom_buffer), a.P);
   if (a.radii == nullptr) a.radii = g.radii;  // rasterizer_impl.cu:381-384
   if (h.accum) {
@@ -485,15 +463,15 @@ int backward_impl(BwdArgs& a, const BwdHost& h) {
 }
 }  // namespace
 
-void set_last_error(const char* msg) { g_err = msg; }
+int fail(const char* entry, const std::string& msg) {
+  g_err = std::string(entry) + ": " + msg;
+  return -1;
+}
+bool kernel_size_ok(float k) { return std::isfinite(k) && k >= 0.f; }
 
 void launch_init_header(ImageHeader* hdr, unsigned long long cap, cudaStream_t st) {
   launch_high_priority(k_init_header, dim3(1), dim3(1), 0, st, hdr, cap);
 }
-
-namespace {
-bool mip_kernel_size_ok(float k) { return std::isfinite(k) && k >= 0.f; }
-}  // namespace
 
 }  // namespace gsr
 
@@ -584,7 +562,7 @@ int64_t gsr_forward_mip(gsr_alloc_fn geometry_alloc, void* geometry_user, gsr_al
                         const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
                         float* out_depth, float* out_median_depth, float* out_opacity, int* radii, int debug,
                         int64_t r_capacity, int64_t* r_host, float kernel_size, void* stream) {
-  if (!mip_kernel_size_ok(kernel_size)) { g_err = "gsr_forward_mip: kernel_size must be finite and >= 0"; return -1; }
+  if (!kernel_size_ok(kernel_size)) return fail("gsr_forward_mip", "kernel_size must be finite and >= 0");
   FwdArgs a{};
   a.P = P; a.D = D; a.M = M; a.W = width; a.H = height; a.prefiltered = prefiltered; a.radii_out = radii;
   a.means3D = means3D; a.shs = shs; a.colors_precomp = colors_precomp; a.opacities = opacities;
@@ -634,8 +612,8 @@ int gsr_backward_mip(int P, int D, int M, int64_t R, const float* background, in
                      float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_ddepth,
                      float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, int debug,
                      const float* opacities, float kernel_size, void* stream) {
-  if (!mip_kernel_size_ok(kernel_size)) { g_err = "gsr_backward_mip: kernel_size must be finite and >= 0"; return -1; }
-  if (P > 0 && !opacities) { g_err = "gsr_backward_mip: opacities are required"; return -1; }
+  if (!kernel_size_ok(kernel_size)) return fail("gsr_backward_mip", "kernel_size must be finite and >= 0");
+  if (P > 0 && !opacities) return fail("gsr_backward_mip", "opacities are required");
   BwdArgs a{};
   a.P = P; a.D = D; a.M = M; a.W = width; a.H = height; a.radii = radii;
   a.means3D = means3D; a.shs = shs; a.colors_precomp = colors_precomp; a.scales = scales; a.rotations = rotations;
@@ -653,124 +631,52 @@ int gsr_backward_mip(int P, int D, int M, int64_t R, const float* background, in
   return backward_impl(a, h);
 }
 
-int gsr_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,
-                     unsigned char* present, void* stream) {
-  if (P <= 0) return 0;
-  launch_mark_visible(P, means3D, viewmatrix, projmatrix, present, (cudaStream_t)stream);
-  return check(cudaGetLastError(), "mark_visible") ? 0 : -1;
-}
-
 int gsr_depth2normal(const float* depth, int width, int height, float fx, float fy, float cx, float cy, float d_min,
                      float d_max, const float* rot, float* out, void* stream) {
   if (width <= 0 || height <= 0) return 0;
-  { Prof pf(kDepth2Normal, (cudaStream_t)stream); launch_depth2normal(depth, width, height, fx, fy, cx, cy, d_min, d_max, rot, out, (cudaStream_t)stream); }
-  return check(cudaGetLastError(), "depth2normal") ? 0 : -1;
+  if (!depth || !out) return fail("gsr_depth2normal", "null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  {
+    Prof pf(kDepth2Normal, st);
+    // K^-1 entries computed on the host in float like torch.inverse of the float32 intrinsics
+    launch_high_priority(k_depth2normal, dim3((width + 31) / 32, (height + 7) / 8), dim3(32, 8), 0, st, depth, width,
+                         height, 1.0f / fx, 1.0f / fy, -cx / fx, -cy / fy, d_min, d_max, rot, out);
+  }
+  return launched("gsr_depth2normal");
 }
 
 int gsr_depth2point(const float* depth, int width, int height, float fx, float fy, float cx, float cy,
                     const float* cam_to_world, float* out, void* stream) {
   if (width <= 0 || height <= 0) return 0;
-  launch_depth2point(depth, width, height, fx, fy, cx, cy, cam_to_world, out, (cudaStream_t)stream);
-  return check(cudaGetLastError(), "depth2point") ? 0 : -1;
-}
-
-int gsr_masked_bilateral(const float* depth, const unsigned char* mask, int width, int height, int d, float sigma_color,
-                         float sigma_space, float* out_depth, unsigned char* out_mask, unsigned int* scratch,
-                         void* stream) {
-  if (width <= 0 || height <= 0) return 0;
-  if (d < 1 || d > 15 || (d & 1) == 0) { g_err = "gsr_masked_bilateral: d must be odd, 1..15"; return -1; }
-  if (!depth || !mask || !out_depth || !out_mask || !scratch) { g_err = "gsr_masked_bilateral: null pointer"; return -1; }
-  // OpenCV: non-positive sigmas become 1; weights are evaluated in double and stored as float
-  const double sc = sigma_color <= 0 ? 1.0 : (double)sigma_color, ss = sigma_space <= 0 ? 1.0 : (double)sigma_space;
-  const double gauss_color = -0.5 / (sc * sc), gauss_space = -0.5 / (ss * ss);
-  const int r = d / 2;
-  SpaceKernel sk;
-  for (int i = 0; i < 225; i++) sk.w[i] = 0.f;
-  for (int dy = -r; dy <= r; dy++)
-    for (int dx = -r; dx <= r; dx++) {
-      const double rr = std::sqrt((double)dy * dy + (double)dx * dx);
-      if (rr > r || (dy == 0 && dx == 0)) continue;
-      sk.w[(dy + r) * (2 * r + 1) + dx + r] = (float)std::exp(rr * rr * gauss_space);
-    }
-  launch_masked_bilateral(depth, mask, width, height, r, (float)gauss_color, sk, out_depth, out_mask, scratch,
-                          (cudaStream_t)stream);
-  return check(cudaGetLastError(), "masked_bilateral") ? 0 : -1;
-}
-
-int gsr_extract_normals(const float* filtered_depth, const unsigned char* fg_mask, const float* opacity,
-                        const float* median_depth, int width, int height, float fx, float fy, float cx, float cy,
-                        const float* rot, float depth_limit, float opacity_min, float* cam_normals,
-                        float* neg_world_normals, unsigned char* valid, void* stream) {
-  if (width <= 0 || height <= 0) return 0;
-  if (!filtered_depth || !fg_mask || !opacity || !median_depth || !rot || !neg_world_normals || !valid) {
-    g_err = "gsr_extract_normals: null pointer"; return -1;
-  }
-  launch_extract_normals(filtered_depth, fg_mask, opacity, median_depth, width, height, fx, fy, cx, cy, rot, depth_limit,
-                         opacity_min, cam_normals, neg_world_normals, valid, (cudaStream_t)stream);
-  return check(cudaGetLastError(), "extract_normals") ? 0 : -1;
-}
-
-int gsr_normal_fusion_pass(int64_t n, const int64_t* ids, const float* normals, const float* confidences, int P,
-                           const float* xyz, float cam_x, float cam_y, float cam_z, const float* mean_normals,
-                           float threshold, float* sum_normals, float* sum_weights, unsigned char* touched,
-                           void* stream) {
-  if (n <= 0) return 0;
-  if (!ids || !normals || !confidences || !xyz || !sum_normals || !sum_weights || P <= 0) {
-    g_err = "gsr_normal_fusion_pass: null pointer"; return -1;
-  }
-  launch_fusion_pass((long long)n, reinterpret_cast<const long long*>(ids), normals, confidences, P, xyz, cam_x, cam_y,
-                     cam_z, mean_normals, threshold, sum_normals, sum_weights, touched, (cudaStream_t)stream);
-  return check(cudaGetLastError(), "normal_fusion_pass") ? 0 : -1;
-}
-
-int gsr_normal_fusion_mean(int P, const float* sum_normals, const float* sum_weights, float* mean_normals, void* stream) {
-  if (P <= 0) return 0;
-  launch_fusion_mean(P, sum_normals, sum_weights, mean_normals, (cudaStream_t)stream);
-  return check(cudaGetLastError(), "normal_fusion_mean") ? 0 : -1;
-}
-
-int gsr_knn_grid(int n, int k, const float* points, const int* cell_start, const float* grid, int* out_index,
-                 float* out_dist, void* stream) {
-  if (n <= 0) return 0;
-  if (!points || !cell_start || !grid || !out_index || !out_dist) { g_err = "gsr_knn_grid: null pointer"; return -1; }
-  if (launch_knn_grid(n, k, points, cell_start, grid, out_index, out_dist, (cudaStream_t)stream) < 0) {
-    g_err = "gsr_knn_grid: k must be 1, 4, 8, 10 or 16";
-    return -1;
-  }
-  return check(cudaGetLastError(), "knn_grid") ? 0 : -1;
-}
-
-int gsr_adam_step(int n_groups, const gsr_adam_group* groups, double beta1, double beta2, double eps, int64_t step,
-                  int decoupled, float grad_scale, int zero_grad, void* stream) {
-  if (n_groups <= 0) return 0;
-  if (!groups || n_groups > GSR_ADAM_MAX_GROUPS) { g_err = "gsr_adam_step: 1..16 groups"; return -1; }
-  if (step < 1) { g_err = "gsr_adam_step: step counts from 1"; return -1; }
-  for (int i = 0; i < n_groups; i++)
-    if (groups[i].numel > 0 && (!groups[i].param || !groups[i].grad || !groups[i].exp_avg || !groups[i].exp_avg_sq)) {
-      g_err = "gsr_adam_step: null tensor in a group"; return -1;
-    }
-  launch_adam(n_groups, groups, beta1, beta2, eps, (long long)step, decoupled, grad_scale, zero_grad, (cudaStream_t)stream);
-  return check(cudaGetLastError(), "adam_step") ? 0 : -1;
+  if (!depth || !out) return fail("gsr_depth2point", "null pointer");
+  k_depth2point<<<dim3((width + 31) / 32, (height + 7) / 8), dim3(32, 8), 0, (cudaStream_t)stream>>>(
+      depth, width, height, 1.0f / fx, 1.0f / fy, -cx / fx, -cy / fy, cam_to_world, out);
+  return launched("gsr_depth2point");
 }
 
 int gsr_debug_export(int P, int width, int height, int64_t R, const char* geom_buffer, const char* binning_buffer,
                      const char* image_buffer, uint32_t* point_list, uint32_t* ranges, uint32_t* n_contrib,
                      float* final_T, float* means2D, float* conic_opacity, float* depths, float* rgb, float* cov3D,
                      uint32_t* tiles_touched, unsigned char* clamped, void* stream) {
+  if (!geom_buffer || !image_buffer || (R > 0 && !binning_buffer))
+    return fail("gsr_debug_export", "missing state buffers");
+  cudaStream_t st = (cudaStream_t)stream;
   GeomView g = carve_geom(aligned_base(const_cast<char*>(geom_buffer)), P);
   ImageView im = carve_image(aligned_base(const_cast<char*>(image_buffer)), width, height);
   BinView b = carve_binning(aligned_base(const_cast<char*>(binning_buffer)), R);
-  launch_debug_export(P, width, height, R, g, b, im, point_list, ranges, n_contrib, final_T, means2D, conic_opacity,
-                      depths, rgb, cov3D, tiles_touched, clamped, (cudaStream_t)stream);
-  return check(cudaGetLastError(), "debug_export") ? 0 : -1;
+  if (P > 0) k_export_geom<<<blocks(P, 256), 256, 0, st>>>(P, g, means2D, conic_opacity, depths, rgb, cov3D, tiles_touched, clamped);
+  if (R > 0 && point_list) k_export_list<<<blocks(R, 256), 256, 0, st>>>(R, im.hdr, b, point_list);
+  const int N = width * height, T = ((width + TILE_X - 1) / TILE_X) * ((height + TILE_Y - 1) / TILE_Y);
+  k_export_image<<<(max(N, T) + 255) / 256, 256, 0, st>>>(N, T, im, ranges, n_contrib, final_T);
+  return launched("gsr_debug_export");
 }
 
 int gsr_debug_accumulator(int P, const char* geom_buffer, float* accum, void* stream) {
-  if (!geom_buffer || !accum) { g_err = "gsr_debug_accumulator: geom_buffer and accum are required"; return -1; }
+  if (!geom_buffer || !accum) return fail("gsr_debug_accumulator", "geom_buffer and accum are required");
   if (P <= 0) return 0;
   GeomView g = carve_geom(aligned_base(const_cast<char*>(geom_buffer)), P);
   return check(cudaMemcpyAsync(accum, g.grad, sizeof(float) * GRAD_F * (size_t)P, cudaMemcpyDeviceToDevice,
-                               (cudaStream_t)stream), "debug_accumulator") ? 0 : -1;
+                               (cudaStream_t)stream), "gsr_debug_accumulator") ? 0 : -1;
 }
 
 int gsr_debug_projection_backward(int fused, int P, int D, int M, int width, int height, const float* means3D,
@@ -782,7 +688,7 @@ int gsr_debug_projection_backward(int fused, int P, int D, int M, int width, int
                                   float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_ddepth,
                                   float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_df_dc,
                                   float* dL_df_rest, float* dL_dscale, float* dL_drot, int debug, void* stream) {
-  if (!accum) { g_err = "gsr_debug_projection_backward: accum is required"; return -1; }
+  if (!accum) return fail("gsr_debug_projection_backward", "accum is required");
   BwdArgs a{};
   a.P = P; a.D = D; a.M = M; a.W = width; a.H = height; a.radii = radii;
   a.fused = fused != 0; a.means3D = means3D; a.scales = scales; a.rotations = rotations;
@@ -810,11 +716,10 @@ int gsr_debug_projection_backward_mip(int P, int D, int M, int width, int height
                                       float* dL_dopacity, float* dL_dcolor, float* dL_ddepth, float* dL_dmean3D,
                                       float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
                                       float kernel_size, int debug, void* stream) {
-  if (!accum) { g_err = "gsr_debug_projection_backward_mip: accum is required"; return -1; }
-  if (!mip_kernel_size_ok(kernel_size)) {
-    g_err = "gsr_debug_projection_backward_mip: kernel_size must be finite and >= 0"; return -1;
-  }
-  if (P > 0 && !opacities) { g_err = "gsr_debug_projection_backward_mip: opacities are required"; return -1; }
+  const char* fn = "gsr_debug_projection_backward_mip";
+  if (!accum) return fail(fn, "accum is required");
+  if (!kernel_size_ok(kernel_size)) return fail(fn, "kernel_size must be finite and >= 0");
+  if (P > 0 && !opacities) return fail(fn, "opacities are required");
   BwdArgs a{};
   a.P = P; a.D = D; a.M = M; a.W = width; a.H = height; a.radii = radii;
   a.means3D = means3D; a.shs = shs; a.colors_precomp = colors_precomp; a.scales = scales; a.rotations = rotations;

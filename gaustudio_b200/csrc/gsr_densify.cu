@@ -198,30 +198,26 @@ extern "C" {
 
 int gsr_densify_stats(int P, const float* viewspace_grad, const int* radii, float* accum, float* denom,
                       float* max_radii2D, void* stream) {
-  if (P < 0) { set_last_error("gsr_densify_stats: P >= 0"); return -1; }
+  if (P < 0) return fail("gsr_densify_stats", "P >= 0");
   if (P == 0) return 0;
-  if (!viewspace_grad || !radii || !accum || !denom || !max_radii2D) {
-    set_last_error("gsr_densify_stats: null pointer"); return -1;
-  }
-  k_densify_stats<<<(P + STATS_THREADS - 1) / STATS_THREADS, STATS_THREADS, 0, (cudaStream_t)stream>>>(
+  if (!viewspace_grad || !radii || !accum || !denom || !max_radii2D) return fail("gsr_densify_stats", "null pointer");
+  k_densify_stats<<<blocks(P, STATS_THREADS), STATS_THREADS, 0, (cudaStream_t)stream>>>(
       P, viewspace_grad, radii, accum, denom, max_radii2D);
-  return check(cudaGetLastError(), "densify_stats") ? 0 : -1;
+  return launched("gsr_densify_stats");
 }
 
 int gsr_densify_count(int P, int scale_dim, const float* accum, const float* denom, const float* scale,
                       const float* opacity, float max_grad, float min_opacity, float clone_max_scale, int prune_big,
                       float big_scale, int* scratch, void* stream) {
-  if (P < 0) { set_last_error("gsr_densify_count: P >= 0"); return -1; }
-  if (scale_dim != 2 && scale_dim != 3) { set_last_error("gsr_densify_count: scale_dim must be 2 or 3"); return -1; }
-  if (!scratch || (P > 0 && (!accum || !denom || !scale || !opacity))) {
-    set_last_error("gsr_densify_count: null pointer"); return -1;
-  }
+  const char* fn = "gsr_densify_count";
+  if (P < 0) return fail(fn, "P >= 0");
+  if (scale_dim != 2 && scale_dim != 3) return fail(fn, "scale_dim must be 2 or 3");
+  if (!scratch || (P > 0 && (!accum || !denom || !scale || !opacity))) return fail(fn, "null pointer");
   if (!std::isfinite(max_grad) || !std::isfinite(min_opacity) || !std::isfinite(clone_max_scale) ||
-      (prune_big && !std::isfinite(big_scale))) {
-    set_last_error("gsr_densify_count: thresholds must be finite"); return -1;
-  }
+      (prune_big && !std::isfinite(big_scale)))
+    return fail(fn, "thresholds must be finite");
   cudaStream_t st = (cudaStream_t)stream;
-  if (P == 0) return check(cudaMemsetAsync(scratch, 0, NCAT * sizeof(int), st), "densify_count") ? 0 : -1;
+  if (P == 0) return check(cudaMemsetAsync(scratch, 0, NCAT * sizeof(int), st), fn) ? 0 : -1;
   const int nb = (P + SCAN_THREADS - 1) / SCAN_THREADS;
   const ScratchView s = carve_scratch(scratch, P, nb);
   CountArgs a{};
@@ -231,54 +227,47 @@ int gsr_densify_count(int P, int scale_dim, const float* accum, const float* den
   k_densify_count<<<nb, SCAN_THREADS, 0, st>>>(a, s, nb);
   k_densify_scan_blocks<<<NCAT, SCAN_THREADS, 0, st>>>(s, nb);
   k_densify_add_blocks<<<nb, SCAN_THREADS, 0, st>>>(P, s, nb);
-  return check(cudaGetLastError(), "densify_count") ? 0 : -1;
+  return launched(fn);
 }
 
 int gsr_densify_apply(int P, int scale_dim, const int* scratch, int n_orig, int n_clone, int n_pair, int n_split,
                       const float* noise, int n_entries, const gsr_densify_entry* entries, void* stream) {
+  const char* fn = "gsr_densify_apply";
   if (P < 0 || n_orig < 0 || n_clone < 0 || n_pair < 0 || n_split < n_pair || n_orig > P || n_clone > P ||
-      n_split > P || (long long)n_orig + n_clone + 2ll * n_pair > 0x7fffffffll) {
-    set_last_error("gsr_densify_apply: counts out of range (P_new = n_orig + n_clone + 2 n_pair must fit in int32)");
-    return -1;
-  }
-  if (scale_dim != 2 && scale_dim != 3) { set_last_error("gsr_densify_apply: scale_dim must be 2 or 3"); return -1; }
-  if (n_entries < 1 || n_entries > GSR_DENSIFY_MAX_ENTRIES || !entries) {
-    set_last_error("gsr_densify_apply: 1..24 entries"); return -1;
-  }
+      n_split > P || (long long)n_orig + n_clone + 2ll * n_pair > 0x7fffffffll)
+    return fail(fn, "counts out of range (P_new = n_orig + n_clone + 2 n_pair must fit in int32)");
+  if (scale_dim != 2 && scale_dim != 3) return fail(fn, "scale_dim must be 2 or 3");
+  if (n_entries < 1 || n_entries > GSR_DENSIFY_MAX_ENTRIES || !entries) return fail(fn, "1..24 entries");
   ApplyTable t{};
   int n_xyz = 0, n_scale = 0, n_rot = 0;
   const bool any_out = (long long)n_orig + n_clone + n_pair > 0;
-  unsigned blocks = 0;
+  unsigned nb = 0;
   for (int k = 0; k < n_entries; k++) {
     const gsr_densify_entry& q = entries[k];
     if (q.role < GSR_DENSIFY_COPY || q.role > GSR_DENSIFY_MOMENT || q.width < 1 || q.width > 4096 ||
         (q.role == GSR_DENSIFY_XYZ && q.width != 3) || (q.role == GSR_DENSIFY_SCALE && q.width != scale_dim) ||
-        (q.role == GSR_DENSIFY_ROT && q.width != 4)) {
-      set_last_error("gsr_densify_apply: bad entry (role, or width: xyz 3, scale scale_dim, rotation 4, others 1..4096)");
-      return -1;
-    }
-    if ((P > 0 && !q.src) || (any_out && !q.dst)) { set_last_error("gsr_densify_apply: null pointer"); return -1; }
+        (q.role == GSR_DENSIFY_ROT && q.width != 4))
+      return fail(fn, "bad entry (role, or width: xyz 3, scale scale_dim, rotation 4, others 1..4096)");
+    if ((P > 0 && !q.src) || (any_out && !q.dst)) return fail(fn, "null pointer");
     n_xyz += q.role == GSR_DENSIFY_XYZ; n_scale += q.role == GSR_DENSIFY_SCALE; n_rot += q.role == GSR_DENSIFY_ROT;
     t.src[k] = q.src; t.dst[k] = q.dst; t.width[k] = q.width; t.role[k] = q.role;
     t.rows_per_block[k] = max(1, APPLY_THREADS * APPLY_ITEMS / q.width);
-    t.first_block[k] = blocks;
-    blocks += (unsigned)((P + t.rows_per_block[k] - 1) / t.rows_per_block[k]);
+    t.first_block[k] = nb;
+    nb += blocks(P, t.rows_per_block[k]);
     if (q.role == GSR_DENSIFY_SCALE) t.scale = q.src;
     if (q.role == GSR_DENSIFY_ROT) t.rot = q.src;
   }
-  if (n_xyz != 1 || n_scale != 1 || n_rot != 1) {
-    set_last_error("gsr_densify_apply: need exactly one xyz, one scale and one rotation entry"); return -1;
-  }
-  if (P > 0 && (!scratch || (n_split > 0 && !noise))) { set_last_error("gsr_densify_apply: null pointer"); return -1; }
-  if (P > 0 && misaligned16(t.rot)) { set_last_error("gsr_densify_apply: rotations must be 16-byte aligned"); return -1; }
+  if (n_xyz != 1 || n_scale != 1 || n_rot != 1) return fail(fn, "need exactly one xyz, one scale and one rotation entry");
+  if (P > 0 && (!scratch || (n_split > 0 && !noise))) return fail(fn, "null pointer");
+  if (P > 0 && misaligned16(t.rot)) return fail(fn, "rotations must be 16-byte aligned");
   if (P == 0 || !any_out) return 0;
-  t.first_block[n_entries] = blocks;
+  t.first_block[n_entries] = nb;
   t.n = n_entries; t.P = P; t.sd = scale_dim; t.n_orig = n_orig; t.n_clone = n_clone; t.n_pair = n_pair;
   t.n_split = n_split; t.noise = noise;
   const ScratchView s = carve_scratch(const_cast<int*>(scratch), P, (P + SCAN_THREADS - 1) / SCAN_THREADS);
   t.pre = s.pre; t.flags = s.flags;
-  k_densify_apply<<<blocks, APPLY_THREADS, 0, (cudaStream_t)stream>>>(t);
-  return check(cudaGetLastError(), "densify_apply") ? 0 : -1;
+  k_densify_apply<<<nb, APPLY_THREADS, 0, (cudaStream_t)stream>>>(t);
+  return launched(fn);
 }
 
 }  // extern "C"

@@ -64,6 +64,8 @@ __global__ void k_dilate_minmax(const float* __restrict__ depth, const unsigned 
 
 __device__ __forceinline__ int reflect101(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
 
+struct SpaceKernel { float w[225]; };  // (2r+1)^2 spatial weights of the bilateral filter, 0 outside the disc
+
 // OpenCV's 32F bilateral filter on (depth - min) / (max - min) with invalid pixels at 0: disc support, centre weight
 // 1, REFLECT_101 border; then filtered * (max - min) + min in separate roundings like the numpy expression.
 __global__ void k_bilateral(const float* __restrict__ depth, const unsigned char* __restrict__ new_mask, int W, int H,
@@ -158,36 +160,6 @@ __global__ void k_fusion_mean(int P, const float* __restrict__ sum_normals, cons
   mean[3 * i] = x / len; mean[3 * i + 1] = y / len; mean[3 * i + 2] = z / len;
 }
 
-void launch_masked_bilateral(const float* depth, const unsigned char* mask, int W, int H, int r, float gauss_color,
-                             const SpaceKernel& sk, float* out_depth, unsigned char* out_mask, unsigned* scratch,
-                             cudaStream_t st) {
-  dim3 blk(32, 8), grd((W + 31) / 32, (H + 7) / 8);
-  k_minmax_init<<<1, 1, 0, st>>>(scratch);
-  k_dilate_minmax<<<grd, blk, 0, st>>>(depth, mask, W, H, r, out_mask, scratch);
-  k_bilateral<<<grd, blk, 0, st>>>(depth, out_mask, W, H, r, gauss_color, sk, scratch, out_depth);
-}
-
-void launch_extract_normals(const float* depth, const unsigned char* fg, const float* opacity, const float* median_depth,
-                            int W, int H, float fx, float fy, float cx, float cy, const float* rot, float depth_limit,
-                            float opacity_min, float* cam_normals, float* neg_world, unsigned char* valid,
-                            cudaStream_t st) {
-  dim3 blk(32, 8), grd((W + 31) / 32, (H + 7) / 8);
-  k_extract_normals<<<grd, blk, 0, st>>>(depth, fg, opacity, median_depth, W, H, 1.0f / fx, 1.0f / fy, -cx / fx, -cy / fy,
-                                         rot, depth_limit, opacity_min, cam_normals, neg_world, valid);
-}
-
-void launch_fusion_pass(long long n, const long long* ids, const float* normals, const float* conf, int P,
-                        const float* xyz, float tx, float ty, float tz, const float* mean, float thresh,
-                        float* sum_normals, float* sum_weights, unsigned char* touched, cudaStream_t st) {
-  if (n <= 0) return;
-  k_fusion_pass<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, ids, normals, conf, P, xyz, tx, ty, tz, mean, thresh,
-                                                             sum_normals, sum_weights, touched);
-}
-
-void launch_fusion_mean(int P, const float* sum_normals, const float* sum_weights, float* mean, cudaStream_t st) {
-  k_fusion_mean<<<(P + 255) / 256, 256, 0, st>>>(P, sum_normals, sum_weights, mean);
-}
-
 }  // namespace gsr
 
 // ---- k nearest neighbours on a uniform grid (neighbour search of extract_pcd.py:170-181, there scipy cKDTree on the host)
@@ -255,111 +227,86 @@ __global__ void __launch_bounds__(128) k_knn_grid(int n, const float* __restrict
   }
 }
 
-int launch_knn_grid(int n, int k, const float* pts, const int* cell_start, const float* grid, int* out_index,
-                    float* out_dist, cudaStream_t st) {
-  const int blocks = (n + 127) / 128;
+}  // namespace gsr
+
+using namespace gsr;
+
+extern "C" {
+
+int gsr_masked_bilateral(const float* depth, const unsigned char* mask, int width, int height, int d, float sigma_color,
+                         float sigma_space, float* out_depth, unsigned char* out_mask, unsigned int* scratch,
+                         void* stream) {
+  if (width <= 0 || height <= 0) return 0;
+  if (d < 1 || d > 15 || (d & 1) == 0) return fail("gsr_masked_bilateral", "d must be odd, 1..15");
+  if (!depth || !mask || !out_depth || !out_mask || !scratch) return fail("gsr_masked_bilateral", "null pointer");
+  // OpenCV: non-positive sigmas become 1; weights are evaluated in double and stored as float
+  const double sc = sigma_color <= 0 ? 1.0 : (double)sigma_color, ss = sigma_space <= 0 ? 1.0 : (double)sigma_space;
+  const double gauss_color = -0.5 / (sc * sc), gauss_space = -0.5 / (ss * ss);
+  const int r = d / 2;
+  SpaceKernel sk;
+  for (int i = 0; i < 225; i++) sk.w[i] = 0.f;
+  for (int dy = -r; dy <= r; dy++)
+    for (int dx = -r; dx <= r; dx++) {
+      const double rr = std::sqrt((double)dy * dy + (double)dx * dx);
+      if (rr > r || (dy == 0 && dx == 0)) continue;
+      sk.w[(dy + r) * (2 * r + 1) + dx + r] = (float)std::exp(rr * rr * gauss_space);
+    }
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 blk(32, 8), grd((width + 31) / 32, (height + 7) / 8);
+  k_minmax_init<<<1, 1, 0, st>>>(scratch);
+  k_dilate_minmax<<<grd, blk, 0, st>>>(depth, mask, width, height, r, out_mask, scratch);
+  k_bilateral<<<grd, blk, 0, st>>>(depth, out_mask, width, height, r, (float)gauss_color, sk, scratch, out_depth);
+  return launched("gsr_masked_bilateral");
+}
+
+int gsr_extract_normals(const float* filtered_depth, const unsigned char* fg_mask, const float* opacity,
+                        const float* median_depth, int width, int height, float fx, float fy, float cx, float cy,
+                        const float* rot, float depth_limit, float opacity_min, float* cam_normals,
+                        float* neg_world_normals, unsigned char* valid, void* stream) {
+  if (width <= 0 || height <= 0) return 0;
+  if (!filtered_depth || !fg_mask || !opacity || !median_depth || !rot || !neg_world_normals || !valid)
+    return fail("gsr_extract_normals", "null pointer");
+  const dim3 blk(32, 8), grd((width + 31) / 32, (height + 7) / 8);
+  k_extract_normals<<<grd, blk, 0, (cudaStream_t)stream>>>(filtered_depth, fg_mask, opacity, median_depth, width, height,
+                                                            1.0f / fx, 1.0f / fy, -cx / fx, -cy / fy, rot, depth_limit,
+                                                            opacity_min, cam_normals, neg_world_normals, valid);
+  return launched("gsr_extract_normals");
+}
+
+int gsr_normal_fusion_pass(int64_t n, const int64_t* ids, const float* normals, const float* confidences, int P,
+                           const float* xyz, float cam_x, float cam_y, float cam_z, const float* mean_normals,
+                           float threshold, float* sum_normals, float* sum_weights, unsigned char* touched,
+                           void* stream) {
+  if (n <= 0) return 0;
+  if (!ids || !normals || !confidences || !xyz || !sum_normals || !sum_weights || P <= 0)
+    return fail("gsr_normal_fusion_pass", "null pointer");
+  k_fusion_pass<<<blocks(n, 256), 256, 0, (cudaStream_t)stream>>>(
+      (long long)n, reinterpret_cast<const long long*>(ids), normals, confidences, P, xyz, cam_x, cam_y, cam_z,
+      mean_normals, threshold, sum_normals, sum_weights, touched);
+  return launched("gsr_normal_fusion_pass");
+}
+
+int gsr_normal_fusion_mean(int P, const float* sum_normals, const float* sum_weights, float* mean_normals, void* stream) {
+  if (P <= 0) return 0;
+  k_fusion_mean<<<blocks(P, 256), 256, 0, (cudaStream_t)stream>>>(P, sum_normals, sum_weights, mean_normals);
+  return launched("gsr_normal_fusion_mean");
+}
+
+int gsr_knn_grid(int n, int k, const float* points, const int* cell_start, const float* grid, int* out_index,
+                 float* out_dist, void* stream) {
+  if (n <= 0) return 0;
+  if (!points || !cell_start || !grid || !out_index || !out_dist) return fail("gsr_knn_grid", "null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  const unsigned nb = blocks(n, 128);
   switch (k) {
-    case 1: k_knn_grid<1><<<blocks, 128, 0, st>>>(n, pts, cell_start, grid, out_index, out_dist); break;
-    case 4: k_knn_grid<4><<<blocks, 128, 0, st>>>(n, pts, cell_start, grid, out_index, out_dist); break;
-    case 8: k_knn_grid<8><<<blocks, 128, 0, st>>>(n, pts, cell_start, grid, out_index, out_dist); break;
-    case 10: k_knn_grid<10><<<blocks, 128, 0, st>>>(n, pts, cell_start, grid, out_index, out_dist); break;
-    case 16: k_knn_grid<16><<<blocks, 128, 0, st>>>(n, pts, cell_start, grid, out_index, out_dist); break;
-    default: return -1;
+    case 1: k_knn_grid<1><<<nb, 128, 0, st>>>(n, points, cell_start, grid, out_index, out_dist); break;
+    case 4: k_knn_grid<4><<<nb, 128, 0, st>>>(n, points, cell_start, grid, out_index, out_dist); break;
+    case 8: k_knn_grid<8><<<nb, 128, 0, st>>>(n, points, cell_start, grid, out_index, out_dist); break;
+    case 10: k_knn_grid<10><<<nb, 128, 0, st>>>(n, points, cell_start, grid, out_index, out_dist); break;
+    case 16: k_knn_grid<16><<<nb, 128, 0, st>>>(n, points, cell_start, grid, out_index, out_dist); break;
+    default: return fail("gsr_knn_grid", "k must be 1, 4, 8, 10 or 16");
   }
-  return 0;
-}
-}  // namespace gsr
-
-// ---------------------------------------------------------------------------------------------------------------
-// Fused multi-tensor Adam / AdamW (SURVEY.md 8f row 3): the reference steps torch.optim.AdamW over five parameter
-// groups (gaustudio/pipelines/optimizers/base.py:19-20, configs/vanilla.yaml:30-46).  One launch updates every
-// group: per element 16 B read (param, grad, exp_avg, exp_avg_sq) and 12-16 B written (the three states, plus the
-// zeroed gradient when zero_grad is fused in) -- a pure HBM stream, float4 wide where the tensors allow it.
-// Arithmetic follows torch's single-tensor Adam: p *= 1 - lr*wd (AdamW) | g += wd*p (Adam); m = m + (g-m)(1-b1);
-// v = v*b2 + (1-b2) g g; p -= (lr/bc1) * m / (sqrt(v)/sqrt(bc2) + eps).
-namespace gsr {
-
-struct AdamTable {
-  float* p[GSR_ADAM_MAX_GROUPS]; float* g[GSR_ADAM_MAX_GROUPS]; float* m[GSR_ADAM_MAX_GROUPS]; float* v[GSR_ADAM_MAX_GROUPS];
-  float* g2[GSR_ADAM_MAX_GROUPS];  // optional second gradient tensor per group (nullptr: none)
-  long long n[GSR_ADAM_MAX_GROUPS];
-  float step_size[GSR_ADAM_MAX_GROUPS], decay[GSR_ADAM_MAX_GROUPS];  // lr / bc1; AdamW: 1 - lr*wd, Adam: wd
-  unsigned first_block[GSR_ADAM_MAX_GROUPS + 1];
-  unsigned char vec4[GSR_ADAM_MAX_GROUPS];
-  int groups;
-};
-constexpr int ADAM_THREADS = 256, ADAM_PER_BLOCK = ADAM_THREADS * 4;
-
-__device__ __forceinline__ void adam_one(float& p, float& g, float& m, float& v, float step_size, float decay, float b1c,
-                                         float b2, float b2c, float inv_bc2s, float eps, float gscale, int decoupled) {
-  float grad = g * gscale;
-  if (decoupled) p = p * decay; else grad = grad + decay * p;
-  m = m + (grad - m) * b1c;
-  v = v * b2 + b2c * grad * grad;
-  const float denom = sqrtf(v) * inv_bc2s + eps;
-  p = p - step_size * (m / denom);
+  return launched("gsr_knn_grid");
 }
 
-__global__ void __launch_bounds__(ADAM_THREADS) k_adam(const __grid_constant__ AdamTable t, float b1c, float b2, float b2c,
-                                                       float inv_bc2s, float eps, float gscale, int decoupled, int zero_grad) {
-  int gi = 0;
-  while (gi + 1 < t.groups && blockIdx.x >= t.first_block[gi + 1]) gi++;
-  const long long base = (long long)(blockIdx.x - t.first_block[gi]) * ADAM_PER_BLOCK;
-  float* __restrict__ P = t.p[gi]; float* __restrict__ G = t.g[gi]; float* __restrict__ M = t.m[gi]; float* __restrict__ V = t.v[gi];
-  float* __restrict__ G2 = t.g2[gi];
-  const long long n = t.n[gi];
-  const float ss = t.step_size[gi], dc = t.decay[gi];
-  const long long i = base + threadIdx.x * 4;
-  if (t.vec4[gi] && i + 3 < n) {
-    float4 p = *reinterpret_cast<float4*>(P + i), g = *reinterpret_cast<float4*>(G + i);
-    float4 m = *reinterpret_cast<float4*>(M + i), v = *reinterpret_cast<float4*>(V + i);
-    if (G2) {
-      const float4 h = *reinterpret_cast<float4*>(G2 + i);
-      g.x += h.x; g.y += h.y; g.z += h.z; g.w += h.w;
-      if (zero_grad) *reinterpret_cast<float4*>(G2 + i) = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    adam_one(p.x, g.x, m.x, v.x, ss, dc, b1c, b2, b2c, inv_bc2s, eps, gscale, decoupled);
-    adam_one(p.y, g.y, m.y, v.y, ss, dc, b1c, b2, b2c, inv_bc2s, eps, gscale, decoupled);
-    adam_one(p.z, g.z, m.z, v.z, ss, dc, b1c, b2, b2c, inv_bc2s, eps, gscale, decoupled);
-    adam_one(p.w, g.w, m.w, v.w, ss, dc, b1c, b2, b2c, inv_bc2s, eps, gscale, decoupled);
-    *reinterpret_cast<float4*>(P + i) = p; *reinterpret_cast<float4*>(M + i) = m; *reinterpret_cast<float4*>(V + i) = v;
-    if (zero_grad) *reinterpret_cast<float4*>(G + i) = make_float4(0.f, 0.f, 0.f, 0.f);
-  } else {
-    for (long long k = i; k < n && k < i + 4; k++) {
-      float p = P[k], g = G[k], m = M[k], v = V[k];
-      if (G2) { g += G2[k]; if (zero_grad) G2[k] = 0.f; }
-      adam_one(p, g, m, v, ss, dc, b1c, b2, b2c, inv_bc2s, eps, gscale, decoupled);
-      P[k] = p; M[k] = m; V[k] = v;
-      if (zero_grad) G[k] = 0.f;
-    }
-  }
-}
-
-int launch_adam(int n_groups, const gsr_adam_group* groups, double beta1, double beta2, double eps, long long step,
-                int decoupled, float grad_scale, int zero_grad, cudaStream_t st) {
-  AdamTable t;
-  const double bc1 = 1.0 - std::pow(beta1, (double)step), bc2 = 1.0 - std::pow(beta2, (double)step);
-  unsigned blocks = 0;
-  int k = 0;
-  for (int i = 0; i < n_groups; i++) {
-    const gsr_adam_group& q = groups[i];
-    if (q.numel <= 0) continue;
-    t.p[k] = q.param; t.g[k] = q.grad; t.m[k] = q.exp_avg; t.v[k] = q.exp_avg_sq; t.n[k] = q.numel;
-    t.step_size[k] = (float)((double)q.lr / bc1);
-    t.decay[k] = decoupled ? (float)(1.0 - (double)q.lr * (double)q.weight_decay) : q.weight_decay;
-    t.g2[k] = q.grad2;
-    t.vec4[k] = ((reinterpret_cast<size_t>(q.param) | reinterpret_cast<size_t>(q.grad) | reinterpret_cast<size_t>(q.exp_avg) |
-                  reinterpret_cast<size_t>(q.exp_avg_sq) | reinterpret_cast<size_t>(q.grad2)) & 15) == 0;
-    t.first_block[k] = blocks;
-    blocks += (unsigned)((q.numel + ADAM_PER_BLOCK - 1) / ADAM_PER_BLOCK);
-    k++;
-  }
-  t.first_block[k] = blocks;
-  t.groups = k;
-  if (!k) return 0;
-  k_adam<<<blocks, ADAM_THREADS, 0, st>>>(t, (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), (float)(1.0 / std::sqrt(bc2)), (float)eps, grad_scale,
-                                          decoupled, zero_grad);
-  return 0;
-}
-
-}  // namespace gsr
+}  // extern "C"

@@ -150,8 +150,6 @@ void launch_preprocess_bwd(const BwdArgs& a, GeomView g, cudaStream_t st);
 // Mip-Splatting projection (2D Mip filter of width kernel_size instead of the 0.3 dilation); un-fused arguments only
 void launch_mip_preprocess_fwd(const FwdArgs& a, GeomView g, ImageView im, float kernel_size, cudaStream_t st);
 void launch_mip_preprocess_bwd(const BwdArgs& a, GeomView g, const float* opacities, float kernel_size, cudaStream_t st);
-void launch_mark_visible(int P, const float* means3D, const float* view, const float* proj,
-                         unsigned char* present, cudaStream_t st);
 // Scaffold-GS anchor visibility (gsr_scaffold_visible, gsr_scaffold.cu): radii[P] of the Mip projection of width
 // kernel_size, un-fused scales [P,3] + rotations [P,4] or cov3D_precomp [P,6]
 struct ScaffoldVisArgs {
@@ -161,14 +159,6 @@ struct ScaffoldVisArgs {
   int* radii;
 };
 void launch_scaffold_visible(const ScaffoldVisArgs& a, cudaStream_t st);
-void launch_depth2normal(const float* depth, int W, int H, float fx, float fy, float cx, float cy, float dmin,
-                         float dmax, const float* rot, float* out, cudaStream_t st);
-void launch_depth2point(const float* depth, int W, int H, float fx, float fy, float cx, float cy, const float* c2w,
-                        float* out, cudaStream_t st);
-void launch_debug_export(int P, int W, int H, long long R, GeomView g, BinView b, ImageView im,
-                         uint32_t* point_list, uint32_t* ranges, uint32_t* n_contrib, float* final_T,
-                         float* means2D, float* conic_opacity, float* depths, float* rgb, float* cov3D,
-                         uint32_t* tiles_touched, unsigned char* clamped, cudaStream_t st);
 
 // ---- small device helpers shared by the kernels ----
 // model activations of gaustudio's VanillaPointCloud (models/vanilla_sg.py:29-35, models/utils.py:6-32)
@@ -334,31 +324,17 @@ __device__ __forceinline__ bool cross_normal(const float* __restrict__ depth, in
   return true;
 }
 
-// gsr_extract.cu -- the extraction post-pass (gaustudio/scripts/extract_pcd.py)
-struct SpaceKernel { float w[225]; };  // (2r+1)^2 spatial weights of the bilateral filter, 0 outside the disc
-void launch_masked_bilateral(const float* depth, const unsigned char* mask, int W, int H, int r, float gauss_color,
-                             const SpaceKernel& sk, float* out_depth, unsigned char* out_mask, unsigned* scratch,
-                             cudaStream_t st);
-void launch_extract_normals(const float* depth, const unsigned char* fg, const float* opacity, const float* median_depth,
-                            int W, int H, float fx, float fy, float cx, float cy, const float* rot, float depth_limit,
-                            float opacity_min, float* cam_normals, float* neg_world, unsigned char* valid,
-                            cudaStream_t st);
-void launch_fusion_pass(long long n, const long long* ids, const float* normals, const float* conf, int P,
-                        const float* xyz, float tx, float ty, float tz, const float* mean, float thresh,
-                        float* sum_normals, float* sum_weights, unsigned char* touched, cudaStream_t st);
-void launch_fusion_mean(int P, const float* sum_normals, const float* sum_weights, float* mean, cudaStream_t st);
-int launch_knn_grid(int n, int k, const float* pts, const int* cell_start, const float* grid, int* out_index,
-                    float* out_dist, cudaStream_t st);  // -1: unsupported k (1, 4, 8, 10, 16)
-}  // namespace gsr
-struct gsr_adam_group;
-namespace gsr {
-int launch_adam(int n_groups, const gsr_adam_group* groups, double beta1, double beta2, double eps, long long step,
-                int decoupled, float grad_scale, int zero_grad, cudaStream_t st);
-
-// the text gsr_last_error() returns next (gsr_api.cu keeps it); for entry points defined in other sources
-void set_last_error(const char* msg);
-
 // ---- host helpers of the entry points ----
+// sets the text gsr_last_error() returns (gsr_api.cu keeps it) to "<entry>: <msg>"; returns -1, the entry's failure
+int fail(const char* entry, const std::string& msg);
+// what an entry returns after its launches: 0, or -1 with the text "<entry>: <CUDA error text>"
+inline int launched(const char* entry) {
+  const cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail(entry, cudaGetErrorString(e));
+}
+inline unsigned blocks(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
+bool kernel_size_ok(float k);  // width of a Mip filter: finite and >= 0
+
 inline size_t align256(size_t v) { return (v + 255) / 256 * 256; }
 // carves `count` elements from p at its next 256-byte boundary and advances p past them
 template <typename T> inline void take(char*& p, T*& out, size_t count) {
@@ -372,7 +348,7 @@ inline bool misaligned16(const void* p) { return (reinterpret_cast<size_t>(p) & 
 
 inline bool check(cudaError_t e, const char* what) {
   if (e == cudaSuccess) return true;
-  set_last_error((std::string(what) + ": " + cudaGetErrorString(e)).c_str());
+  fail(what, cudaGetErrorString(e));
   return false;
 }
 // CHECK_CUDA of the reference (auxiliary.h:166-173): with debug, synchronise and surface errors per stage

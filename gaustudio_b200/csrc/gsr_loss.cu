@@ -213,20 +213,11 @@ __global__ void __launch_bounds__(THREADS) k_ssim_bwd(const SsimBwdArgs a) {
 
 // the checks every entry point makes before any work; -> number of CTAs, or -1 with the error text set
 long long ssim_grid(const char* entry, long long planes, int H, int W) {
-  if (planes < 1 || H < 1 || W < 1) {
-    set_last_error((std::string(entry) + ": planes, H and W must be >= 1").c_str());
-    return -1;
-  }
+  if (planes < 1 || H < 1 || W < 1) return fail(entry, "planes, H and W must be >= 1");
   // 3 * planes * H * W: the elements of the D maps
-  if (planes > INT64_MAX / 3 / H / W) {
-    set_last_error((std::string(entry) + ": element count overflows int64").c_str());
-    return -1;
-  }
+  if (planes > INT64_MAX / 3 / H / W) return fail(entry, "element count overflows int64");
   const long long tiles = (long long)((W + TX - 1) / TX) * ((H + TY - 1) / TY);
-  if (planes > 0x7fffffffll / tiles) {
-    set_last_error((std::string(entry) + ": too many tiles for one grid (planes x tiles must fit in int32)").c_str());
-    return -1;
-  }
+  if (planes > 0x7fffffffll / tiles) return fail(entry, "too many tiles for one grid (planes x tiles must fit in int32)");
   return planes * tiles;
 }
 
@@ -247,28 +238,26 @@ int gsr_ssim_forward(int64_t planes, int H, int W, const float* img1, const floa
                      void* scratch, float* sums, void* stream) {
   const long long n = ssim_grid("gsr_ssim_forward", planes, H, W);
   if (n < 0) return -1;
-  if (!img1 || !img2 || !scratch || !sums) { set_last_error("gsr_ssim_forward: null pointer"); return -1; }
+  if (!img1 || !img2 || !scratch || !sums) return fail("gsr_ssim_forward", "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   SsimFwdArgs a{};
   a.H = H; a.W = W; a.plane_px = (long long)H * W; a.maps_stride = planes * a.plane_px;
   a.x = img1; a.y = img2; a.maps = partials; a.cta_sums = (double*)scratch;
   k_ssim_fwd<<<(unsigned)n, THREADS, 0, st>>>(a);
   k_ssim_reduce<<<1, REDUCE_THREADS, 0, st>>>(a.cta_sums, (int)n, sums);
-  return check(cudaGetLastError(), "ssim_forward") ? 0 : -1;
+  return launched("gsr_ssim_forward");
 }
 
 int gsr_ssim_backward(int64_t planes, int H, int W, const float* img1, const float* img2, const float* partials,
                       const float* d_sums, float* d_img1, void* stream) {
   const long long n = ssim_grid("gsr_ssim_backward", planes, H, W);
   if (n < 0) return -1;
-  if (!img1 || !img2 || !partials || !d_sums || !d_img1) {
-    set_last_error("gsr_ssim_backward: null pointer"); return -1;
-  }
+  if (!img1 || !img2 || !partials || !d_sums || !d_img1) return fail("gsr_ssim_backward", "null pointer");
   SsimBwdArgs a{};
   a.H = H; a.W = W; a.plane_px = (long long)H * W; a.maps_stride = planes * a.plane_px;
   a.x = img1; a.y = img2; a.maps = partials; a.d_sums = d_sums; a.d_x = d_img1;
   k_ssim_bwd<<<(unsigned)n, THREADS, 0, (cudaStream_t)stream>>>(a);
-  return check(cudaGetLastError(), "ssim_backward") ? 0 : -1;
+  return launched("gsr_ssim_backward");
 }
 
 }  // extern "C"

@@ -402,16 +402,9 @@ __global__ void k_label(long long F, int* parent, long long* __restrict__ labels
   if (f < F) labels[f] = uf_find(parent, (int)f);
 }
 
-inline unsigned blocks(long long n, int t) { return (unsigned)((n + t - 1) / t); }
-bool cuda_ok(const char* what) {
-  const cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess) return true;
-  set_last_error((std::string(what) + ": " + cudaGetErrorString(e)).c_str());
-  return false;
-}
 bool cap_ok(const char* fn, long long cap) {
   if (cap >= 1 && cap <= MAX_CAPACITY) return true;
-  set_last_error((std::string(fn) + ": capacity_bricks must be in 1..262144").c_str());
+  fail(fn, "capacity_bricks must be in 1..262144");
   return false;
 }
 
@@ -430,7 +423,7 @@ bool sort_bricks(const char* fn, const TsdfView& v, gsr_alloc_fn alloc, void* us
   const size_t o_keys = 0, o_iota = align256((size_t)cap * 8), o_idx = o_iota + align256((size_t)cap * 4),
                o_tmp = o_idx + align256((size_t)cap * 4), o_rest = o_tmp + align256(sort_tmp);
   char* s = alloc(user, o_rest + extra);
-  if (!s) { set_last_error((std::string(fn) + ": scratch allocation failed").c_str()); return false; }
+  if (!s) { fail(fn, "scratch allocation failed"); return false; }
   out.keys = reinterpret_cast<unsigned long long*>(s + o_keys);
   out.idx = reinterpret_cast<int*>(s + o_idx);
   out.rest = s + o_rest;
@@ -438,19 +431,17 @@ bool sort_bricks(const char* fn, const TsdfView& v, gsr_alloc_fn alloc, void* us
   k_iota<<<blocks(cap, 256), 256, 0, st>>>(cap, iota);
   cub::DeviceRadixSort::SortPairs(s + o_tmp, sort_tmp, (const unsigned long long*)v.brick_keys, out.keys,
                                   (const int*)iota, out.idx, cap, 0, 64, st);
-  return cuda_ok(fn);
+  return launched(fn) == 0;
 }
 
 bool volume_ok(const char* fn, const unsigned long long* rb, long long cap) {
   if (rb[0] > (unsigned long long)cap || rb[1]) {
-    set_last_error((std::string(fn) + ": the TSDF volume needs " + (rb[1] ? "more than " : "") +
-                    std::to_string(rb[0]) + " bricks but its capacity is " + std::to_string(cap) +
-                    " (create it with a larger capacity_bricks)").c_str());
+    fail(fn, (rb[1] ? "the TSDF volume needs more than " : "the TSDF volume needs ") + std::to_string(rb[0]) +
+                 " bricks but its capacity is " + std::to_string(cap) + " (create it with a larger capacity_bricks)");
     return false;
   }
   if (rb[2]) {
-    set_last_error((std::string(fn) + ": " + std::to_string(rb[2]) +
-                    " samples or rays fell outside the addressable range (|voxel index| < 2^23)").c_str());
+    fail(fn, std::to_string(rb[2]) + " samples or rays fell outside the addressable range (|voxel index| < 2^23)");
     return false;
   }
   return true;
@@ -469,12 +460,11 @@ size_t gsr_tsdf_bytes(int64_t capacity_bricks) {
 }
 
 int gsr_tsdf_init(void* state, int64_t capacity_bricks, double voxel_size, double sdf_trunc, void* stream) {
-  if (!state) { set_last_error("gsr_tsdf_init: state is required"); return -1; }
-  if (!cap_ok("gsr_tsdf_init", capacity_bricks)) return -1;
-  if (!(voxel_size > 0.0 && voxel_size < 1e30 && sdf_trunc > 0.0 && sdf_trunc < 1e30)) {
-    set_last_error("gsr_tsdf_init: voxel_size and sdf_trunc must be positive and finite");
-    return -1;
-  }
+  const char* fn = "gsr_tsdf_init";
+  if (!state) return fail(fn, "state is required");
+  if (!cap_ok(fn, capacity_bricks)) return -1;
+  if (!(voxel_size > 0.0 && voxel_size < 1e30 && sdf_trunc > 0.0 && sdf_trunc < 1e30))
+    return fail(fn, "voxel_size and sdf_trunc must be positive and finite");
   cudaStream_t st = (cudaStream_t)stream;
   TsdfView v;
   char* base = static_cast<char*>(state);
@@ -484,39 +474,35 @@ int gsr_tsdf_init(void* state, int64_t capacity_bricks, double voxel_size, doubl
   cudaMemsetAsync(base + 256, 0xff, keys_end - 256, st);  // table keys, slot bricks, brick keys: all "empty"
   cudaMemsetAsync(v.sums, 0, bytes - keys_end, st);
   k_init_header<<<1, 1, 0, st>>>(v.hdr, voxel_size, sdf_trunc);
-  return cuda_ok("gsr_tsdf_init") ? 0 : -1;
+  return launched(fn);
 }
 
 int gsr_tsdf_integrate(void* state, int64_t capacity_bricks, int64_t n, const float* points,
                        const unsigned char* valid, double origin_x, double origin_y, double origin_z, void* stream) {
-  if (!state) { set_last_error("gsr_tsdf_integrate: state is required"); return -1; }
-  if (!cap_ok("gsr_tsdf_integrate", capacity_bricks)) return -1;
-  if (n < 0) { set_last_error("gsr_tsdf_integrate: n must be >= 0"); return -1; }
-  if (n > 0 && !points) { set_last_error("gsr_tsdf_integrate: points is required"); return -1; }
-  if (!(std::fabs(origin_x) < 1e300 && std::fabs(origin_y) < 1e300 && std::fabs(origin_z) < 1e300)) {
-    set_last_error("gsr_tsdf_integrate: origin must be finite");
-    return -1;
-  }
+  const char* fn = "gsr_tsdf_integrate";
+  if (!state) return fail(fn, "state is required");
+  if (!cap_ok(fn, capacity_bricks)) return -1;
+  if (n < 0) return fail(fn, "n must be >= 0");
+  if (n > 0 && !points) return fail(fn, "points is required");
+  if (!(std::fabs(origin_x) < 1e300 && std::fabs(origin_y) < 1e300 && std::fabs(origin_z) < 1e300))
+    return fail(fn, "origin must be finite");
   if (n == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   TsdfView v;
   tsdf_layout(static_cast<char*>(state), capacity_bricks, &v);
   k_tsdf_rays<false><<<blocks(n, 128), 128, 0, st>>>(v, n, points, valid, origin_x, origin_y, origin_z);
   k_tsdf_rays<true><<<blocks(n, 128), 128, 0, st>>>(v, n, points, valid, origin_x, origin_y, origin_z);
-  return cuda_ok("gsr_tsdf_integrate") ? 0 : -1;
+  return launched(fn);
 }
 
 int64_t gsr_tsdf_extract(void* state, int64_t capacity_bricks, double min_weight, gsr_alloc_fn scratch_alloc,
                          void* scratch_user, gsr_alloc_fn vertex_alloc, void* vertex_user, gsr_alloc_fn face_alloc,
                          void* face_user, int64_t* n_faces, void* stream) {
   const char* fn = "gsr_tsdf_extract";
-  if (!state) { set_last_error("gsr_tsdf_extract: state is required"); return -1; }
+  if (!state) return fail(fn, "state is required");
   if (!cap_ok(fn, capacity_bricks)) return -1;
-  if (!(min_weight >= 0.0)) { set_last_error("gsr_tsdf_extract: min_weight must be >= 0"); return -1; }
-  if (!scratch_alloc || !vertex_alloc || !face_alloc || !n_faces) {
-    set_last_error("gsr_tsdf_extract: allocators and n_faces are required");
-    return -1;
-  }
+  if (!(min_weight >= 0.0)) return fail(fn, "min_weight must be >= 0");
+  if (!scratch_alloc || !vertex_alloc || !face_alloc || !n_faces) return fail(fn, "allocators and n_faces are required");
   cudaStream_t st = (cudaStream_t)stream;
   TsdfView v;
   tsdf_layout(static_cast<char*>(state), capacity_bricks, &v);
@@ -547,26 +533,26 @@ int64_t gsr_tsdf_extract(void* state, int64_t capacity_bricks, double min_weight
   k_readback<<<1, 1, 0, st>>>(v, vbase, fbase, N, rb_dev);
   unsigned long long rb[5];
   cudaMemcpyAsync(rb, rb_dev, sizeof(rb), cudaMemcpyDeviceToHost, st);
-  if (!cuda_ok(fn)) return -1;
-  if (cudaStreamSynchronize(st) != cudaSuccess) { cuda_ok(fn); return -1; }
+  if (launched(fn)) return -1;
+  if (cudaStreamSynchronize(st) != cudaSuccess) { launched(fn); return -1; }
   if (!volume_ok(fn, rb, capacity_bricks)) return -1;
   const long long V = (long long)rb[3], F = (long long)rb[4];
   *n_faces = F;
   if (V == 0 && F == 0) return 0;
   char* verts = vertex_alloc(vertex_user, (size_t)V * 12);
   char* faces = face_alloc(face_user, (size_t)F * 24);
-  if (!verts || !faces) { set_last_error("gsr_tsdf_extract: output allocation failed"); return -1; }
+  if (!verts || !faces) return fail(fn, "output allocation failed");
   k_mc_emit<<<blocks(N, 128), 128, 0, st>>>(m, N, fbase, reinterpret_cast<float*>(verts),
                                             reinterpret_cast<long long*>(faces));
-  return cuda_ok(fn) ? V : -1;
+  return launched(fn) ? -1 : V;
 }
 
 int64_t gsr_tsdf_export(void* state, int64_t capacity_bricks, gsr_alloc_fn scratch_alloc, void* scratch_user,
                         int64_t* brick_keys, int64_t* sums, int* weights, void* stream) {
   const char* fn = "gsr_tsdf_export";
-  if (!state) { set_last_error("gsr_tsdf_export: state is required"); return -1; }
+  if (!state) return fail(fn, "state is required");
   if (!cap_ok(fn, capacity_bricks)) return -1;
-  if (!scratch_alloc) { set_last_error("gsr_tsdf_export: scratch_alloc is required"); return -1; }
+  if (!scratch_alloc) return fail(fn, "scratch_alloc is required");
   cudaStream_t st = (cudaStream_t)stream;
   TsdfView v;
   tsdf_layout(static_cast<char*>(state), capacity_bricks, &v);
@@ -576,31 +562,23 @@ int64_t gsr_tsdf_export(void* state, int64_t capacity_bricks, gsr_alloc_fn scrat
   k_readback<<<1, 1, 0, st>>>(v, nullptr, nullptr, 0, rb_dev);
   unsigned long long rb[5];
   cudaMemcpyAsync(rb, rb_dev, sizeof(rb), cudaMemcpyDeviceToHost, st);
-  if (!cuda_ok(fn)) return -1;
-  if (cudaStreamSynchronize(st) != cudaSuccess) { cuda_ok(fn); return -1; }
+  if (launched(fn)) return -1;
+  if (cudaStreamSynchronize(st) != cudaSuccess) { launched(fn); return -1; }
   if (!volume_ok(fn, rb, capacity_bricks)) return -1;
   const long long n = (long long)rb[0];
   if (n > 0 && (brick_keys || sums || weights))
     k_export<<<(unsigned)n, 256, 0, st>>>(v, sb.keys, sb.idx, reinterpret_cast<long long*>(brick_keys),
                                           reinterpret_cast<long long*>(sums), weights);
-  return cuda_ok(fn) ? n : -1;
+  return launched(fn) ? -1 : n;
 }
 
 int gsr_mesh_face_components(int64_t n_faces, const int64_t* faces, int64_t n_vertices, gsr_alloc_fn scratch_alloc,
                              void* scratch_user, int64_t* labels, void* stream) {
-  if (n_faces < 0 || n_faces > (1LL << 29)) {
-    set_last_error("gsr_mesh_face_components: n_faces must be in 0..2^29");
-    return -1;
-  }
-  if (n_vertices < 0 || n_vertices > (1LL << 31)) {
-    set_last_error("gsr_mesh_face_components: n_vertices must be in 0..2^31");
-    return -1;
-  }
+  const char* fn = "gsr_mesh_face_components";
+  if (n_faces < 0 || n_faces > (1LL << 29)) return fail(fn, "n_faces must be in 0..2^29");
+  if (n_vertices < 0 || n_vertices > (1LL << 31)) return fail(fn, "n_vertices must be in 0..2^31");
   if (n_faces == 0) return 0;
-  if (!faces || !labels || !scratch_alloc) {
-    set_last_error("gsr_mesh_face_components: faces, labels and scratch_alloc are required");
-    return -1;
-  }
+  if (!faces || !labels || !scratch_alloc) return fail(fn, "faces, labels and scratch_alloc are required");
   cudaStream_t st = (cudaStream_t)stream;
   const long long F = n_faces, n = 3 * F;
   size_t sort_tmp = 0;
@@ -609,7 +587,7 @@ int gsr_mesh_face_components(int64_t n_faces, const int64_t* faces, int64_t n_ve
   const size_t o_k = 0, o_v = align256(n * 8), o_k2 = o_v + align256(n * 4), o_v2 = o_k2 + align256(n * 8),
                o_p = o_v2 + align256(n * 4), o_t = o_p + align256(F * 4), total = o_t + align256(sort_tmp);
   char* s = scratch_alloc(scratch_user, total);
-  if (!s) { set_last_error("gsr_mesh_face_components: scratch allocation failed"); return -1; }
+  if (!s) return fail(fn, "scratch allocation failed");
   auto* keys = reinterpret_cast<unsigned long long*>(s + o_k);
   auto* vals = reinterpret_cast<int*>(s + o_v);
   auto* keys2 = reinterpret_cast<unsigned long long*>(s + o_k2);
@@ -621,7 +599,7 @@ int gsr_mesh_face_components(int64_t n_faces, const int64_t* faces, int64_t n_ve
   k_iota<<<blocks(F, 256), 256, 0, st>>>((int)F, parent);
   k_union<<<blocks(n, 256), 256, 0, st>>>(n, keys2, vals2, parent);
   k_label<<<blocks(F, 256), 256, 0, st>>>(F, parent, reinterpret_cast<long long*>(labels));
-  return cuda_ok("gsr_mesh_face_components") ? 0 : -1;
+  return launched(fn);
 }
 
 }  // extern "C"

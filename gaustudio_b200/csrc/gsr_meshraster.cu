@@ -17,7 +17,6 @@
 #include "../../include/gsr.h"
 #include <cub/cub.cuh>
 #include <cmath>
-#include <string>
 
 namespace gsr {
 namespace {
@@ -371,29 +370,18 @@ __global__ void __launch_bounds__(256) k_tex_vertices(MeshCam cam, const float* 
   }
 }
 
-inline unsigned blocks(long long n, int t) { return (unsigned)((n + t - 1) / t); }
-bool cuda_ok(const char* what) {
-  const cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess) return true;
-  set_last_error((std::string(what) + ": " + cudaGetErrorString(e)).c_str());
-  return false;
-}
-bool fail(const char* fn, const char* msg) {
-  set_last_error((std::string(fn) + ": " + msg).c_str());
-  return false;
-}
 constexpr long long MAX_COUNT = 2147483647LL;
 
-// The checks every entry point shares, in this order: counts, image size, camera.  False with the error set.
-bool common_ok(const char* fn, long long V, long long F, int W, int H, const double* camera, double fx, double fy,
-               double cx, double cy) {
-  if (V < 0 || V > MAX_COUNT || F < 0 || F > MAX_COUNT) return fail(fn, "n_vertices and n_faces must be in 0..2^31-1");
-  if (W < 1 || W > MAX_SIDE || H < 1 || H > MAX_SIDE) return fail(fn, "width and height must be in 1..32768");
-  if (!camera) return fail(fn, "camera is required");
+// The checks every entry point shares, in this order: counts, image size, camera.  The message, or nullptr.
+const char* common_error(long long V, long long F, int W, int H, const double* camera, double fx, double fy, double cx,
+                         double cy) {
+  if (V < 0 || V > MAX_COUNT || F < 0 || F > MAX_COUNT) return "n_vertices and n_faces must be in 0..2^31-1";
+  if (W < 1 || W > MAX_SIDE || H < 1 || H > MAX_SIDE) return "width and height must be in 1..32768";
+  if (!camera) return "camera is required";
   bool finite = std::isfinite(fx) && std::isfinite(fy) && std::isfinite(cx) && std::isfinite(cy);
   for (int i = 0; i < 12; i++) finite = finite && std::isfinite(camera[i]);
-  if (!finite) return fail(fn, "camera, fx, fy, cx and cy must be finite");
-  return true;
+  if (!finite) return "camera, fx, fy, cx and cy must be finite";
+  return nullptr;
 }
 MeshCam make_cam(const double* camera, double fx, double fy, double cx, double cy, double znear, int W, int H) {
   MeshCam c;
@@ -430,14 +418,12 @@ int gsr_mesh_rasterize(int64_t n_vertices, const float* vertices, int64_t n_face
                        const double* camera, double fx, double fy, double cx, double cy, double znear, int width,
                        int height, void* scratch, size_t scratch_bytes, int* face_id, float* depth, void* stream) {
   const char* fn = "gsr_mesh_rasterize";
-  if (!common_ok(fn, n_vertices, n_faces, width, height, camera, fx, fy, cx, cy)) return -1;
-  if (!(znear >= 0.0 && std::isfinite(znear))) { fail(fn, "znear must be finite and >= 0"); return -1; }
-  if ((n_vertices > 0 && !vertices) || (n_faces > 0 && !faces) || !face_id || !depth || !scratch) {
-    fail(fn, "vertices, faces, scratch, face_id and depth are required");
-    return -1;
-  }
+  if (const char* e = common_error(n_vertices, n_faces, width, height, camera, fx, fy, cx, cy)) return fail(fn, e);
+  if (!(znear >= 0.0 && std::isfinite(znear))) return fail(fn, "znear must be finite and >= 0");
+  if ((n_vertices > 0 && !vertices) || (n_faces > 0 && !faces) || !face_id || !depth || !scratch)
+    return fail(fn, "vertices, faces, scratch, face_id and depth are required");
   const RasterLayout L = raster_layout(n_vertices, n_faces, width, height);
-  if (scratch_bytes < L.total) { fail(fn, "scratch is smaller than gsr_mesh_raster_bytes"); return -1; }
+  if (scratch_bytes < L.total) return fail(fn, "scratch is smaller than gsr_mesh_raster_bytes");
   cudaStream_t st = (cudaStream_t)stream;
   char* s = static_cast<char*>(scratch);
   RasterCtx c;
@@ -459,7 +445,7 @@ int gsr_mesh_rasterize(int64_t n_vertices, const float* vertices, int64_t n_face
   }
   const long long n = (long long)width * height;
   k_mr_resolve<<<blocks(n, 256), 256, 0, st>>>(n, c.keys, face_id, depth);
-  return cuda_ok(fn) ? 0 : -1;
+  return launched(fn);
 }
 
 int gsr_mesh_shade(int64_t n_vertices, const float* vertices, int64_t n_faces, const int64_t* faces,
@@ -467,18 +453,16 @@ int gsr_mesh_shade(int64_t n_vertices, const float* vertices, int64_t n_faces, c
                    const int* face_id, const float* vertex_normals, const float* vertex_colors, float* normal,
                    float* color, void* stream) {
   const char* fn = "gsr_mesh_shade";
-  if (!common_ok(fn, n_vertices, n_faces, width, height, camera, fx, fy, cx, cy)) return -1;
-  if (!face_id || (n_faces > 0 && !faces) || (n_vertices > 0 && !vertices)) {
-    fail(fn, "vertices, faces and face_id are required");
-    return -1;
-  }
-  if (normal && n_vertices > 0 && !vertex_normals) { fail(fn, "a normal map needs vertex_normals"); return -1; }
+  if (const char* e = common_error(n_vertices, n_faces, width, height, camera, fx, fy, cx, cy)) return fail(fn, e);
+  if (!face_id || (n_faces > 0 && !faces) || (n_vertices > 0 && !vertices))
+    return fail(fn, "vertices, faces and face_id are required");
+  if (normal && n_vertices > 0 && !vertex_normals) return fail(fn, "a normal map needs vertex_normals");
   if (!normal && !color) return 0;
   const long long n = (long long)width * height;
   k_mr_shade<<<blocks(n, 256), 256, 0, (cudaStream_t)stream>>>(
       make_cam(camera, fx, fy, cx, cy, 0.0, width, height), vertices, n_vertices,
       reinterpret_cast<const long long*>(faces), n_faces, face_id, vertex_normals, vertex_colors, normal, color);
-  return cuda_ok(fn) ? 0 : -1;
+  return launched(fn);
 }
 
 int gsr_mesh_texture_view(int64_t n_vertices, const float* vertices, int64_t n_faces, const int64_t* faces,
@@ -486,13 +470,11 @@ int gsr_mesh_texture_view(int64_t n_vertices, const float* vertices, int64_t n_f
                           const int* face_id, const float* image, int view, int* face_stamp, int* vertex_stamp,
                           int64_t* stats, float* vertex_colors, void* stream) {
   const char* fn = "gsr_mesh_texture_view";
-  if (!common_ok(fn, n_vertices, n_faces, width, height, camera, fx, fy, cx, cy)) return -1;
-  if (view < 0 || view >= 2147483647) { fail(fn, "view must be in 0..2^31-2"); return -1; }
+  if (const char* e = common_error(n_vertices, n_faces, width, height, camera, fx, fy, cx, cy)) return fail(fn, e);
+  if (view < 0 || view >= 2147483647) return fail(fn, "view must be in 0..2^31-2");
   if (!face_id || !image || !face_stamp || !vertex_stamp || !stats || !vertex_colors ||
-      (n_faces > 0 && !faces) || (n_vertices > 0 && !vertices)) {
-    fail(fn, "vertices, faces, face_id, image, face_stamp, vertex_stamp, stats and vertex_colors are required");
-    return -1;
-  }
+      (n_faces > 0 && !faces) || (n_vertices > 0 && !vertices))
+    return fail(fn, "vertices, faces, face_id, image, face_stamp, vertex_stamp, stats and vertex_colors are required");
   if (n_faces == 0 || n_vertices == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   const MeshCam cam = make_cam(camera, fx, fy, cx, cy, 0.0, width, height);
@@ -503,7 +485,7 @@ int gsr_mesh_texture_view(int64_t n_vertices, const float* vertices, int64_t n_f
                                                      vertex_stamp, reinterpret_cast<unsigned long long*>(stats));
   k_tex_vertices<<<blocks(n_vertices, 256), 256, 0, st>>>(cam, vertices, n_vertices, view + 1, vertex_stamp, image,
                                                           vertex_colors);
-  return cuda_ok(fn) ? 0 : -1;
+  return launched(fn);
 }
 
 }  // extern "C"

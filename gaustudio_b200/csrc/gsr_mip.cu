@@ -79,21 +79,14 @@ using namespace gsr;
 
 extern "C" int gsr_mip_filter3d(int P, const float* means3D, int n_cameras, const float* cameras, float* filter_3D,
                                 unsigned int* scratch, void* stream) {
-  if (P < 0 || n_cameras < 0) { set_last_error("gsr_mip_filter3d: P and n_cameras must be >= 0"); return -1; }
+  const char* fn = "gsr_mip_filter3d";
+  if (P < 0 || n_cameras < 0) return fail(fn, "P and n_cameras must be >= 0");
   if (P == 0) return 0;
-  if (!means3D || !filter_3D || !scratch || (n_cameras > 0 && !cameras)) {
-    set_last_error("gsr_mip_filter3d: null pointer");
-    return -1;
-  }
+  if (!means3D || !filter_3D || !scratch || (n_cameras > 0 && !cameras)) return fail(fn, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  if (cudaMemsetAsync(scratch, 0, 3 * sizeof(unsigned), st) != cudaSuccess) {
-    set_last_error("gsr_mip_filter3d: memset scratch failed");
-    return -1;
-  }
-  const unsigned blocks = (unsigned)((P + F3_THREADS - 1) / F3_THREADS);
-  k_mip_filter3d_min<<<blocks, F3_THREADS, 0, st>>>(P, means3D, n_cameras, cameras, filter_3D, scratch);
-  k_mip_filter3d_fill<<<blocks, F3_THREADS, 0, st>>>(P, filter_3D, scratch);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(cudaGetErrorString(e)); return -1; }
-  return 0;
+  if (cudaMemsetAsync(scratch, 0, 3 * sizeof(unsigned), st) != cudaSuccess) return fail(fn, "memset scratch failed");
+  const unsigned nb = blocks(P, F3_THREADS);
+  k_mip_filter3d_min<<<nb, F3_THREADS, 0, st>>>(P, means3D, n_cameras, cameras, filter_3D, scratch);
+  k_mip_filter3d_fill<<<nb, F3_THREADS, 0, st>>>(P, filter_3D, scratch);
+  return launched(fn);
 }

@@ -8,6 +8,7 @@
 // Design differences (H100): one packed 48-B splat record per Gaussian instead of five SoA arrays; per-tile
 // instance counts are accumulated here (no per-Gaussian prefix scan, no duplicateWithKeys offsets); K6 and
 // K7 are one kernel and write every output element (no torch::zeros pre-pass, rasterize_points.cu:160-169).
+#include "../../include/gsr.h"
 #include "gsr_internal.cuh"
 
 #include <cstdio>
@@ -856,10 +857,6 @@ void launch_mip_preprocess_bwd(const BwdArgs& a, GeomView g, const float* opacit
   launch_high_priority(k_mip_preprocess_bwd, dim3((a.P + PRE_THREADS - 1) / PRE_THREADS), dim3(PRE_THREADS), smem, st,
                        a, g, opacities, kernel_size);
 }
-void launch_mark_visible(int P, const float* means3D, const float* view, const float*, unsigned char* present,
-                         cudaStream_t st) {
-  k_mark_visible<<<(P + 255) / 256, 256, 0, st>>>(P, means3D, view, present);
-}
 // focal lengths and tile grid from the host expressions of forward_impl (gsr_api.cu), so they are the same floats
 void launch_scaffold_visible(const ScaffoldVisArgs& a, cudaStream_t st) {
   const float focal_y = a.H / (2.0f * a.tan_fovy), focal_x = a.W / (2.0f * a.tan_fovx);
@@ -868,3 +865,15 @@ void launch_scaffold_visible(const ScaffoldVisArgs& a, cudaStream_t st) {
 }
 
 }  // namespace gsr
+
+using namespace gsr;
+
+// Rasterizer::markVisible (rasterizer_impl.cu:141-153); projmatrix is not read: the test is the view-space near plane
+extern "C" int gsr_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,
+                                unsigned char* present, void* stream) {
+  (void)projmatrix;
+  if (P <= 0) return 0;
+  if (!means3D || !viewmatrix || !present) return fail("gsr_mark_visible", "null pointer");
+  k_mark_visible<<<blocks(P, 256), 256, 0, (cudaStream_t)stream>>>(P, means3D, viewmatrix, present);
+  return launched("gsr_mark_visible");
+}

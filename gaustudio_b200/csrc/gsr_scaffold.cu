@@ -10,8 +10,6 @@
 #include "../../include/gsr.h"
 #include "gsr_internal.cuh"
 
-#include <cmath>
-
 namespace gsr {
 
 namespace {
@@ -177,18 +175,13 @@ int gsr_scaffold_visible(int N, const float* means3D, const float* scales, const
                          const float* cov3D_precomp, float scale_modifier, const float* viewmatrix,
                          const float* projmatrix, int width, int height, float tan_fovx, float tan_fovy,
                          float kernel_size, int* radii, void* stream) {
-  if (N < 0 || width <= 0 || height <= 0) { set_last_error("gsr_scaffold_visible: N >= 0, width and height > 0"); return -1; }
-  if (!(std::isfinite(kernel_size) && kernel_size >= 0.f)) {
-    set_last_error("gsr_scaffold_visible: kernel_size must be finite and >= 0"); return -1;
-  }
-  if (!means3D || !viewmatrix || !projmatrix || !radii || (!cov3D_precomp && (!scales || !rotations))) {
-    set_last_error("gsr_scaffold_visible: need means3D, the camera, radii and scales+rotations or cov3D_precomp");
-    return -1;
-  }
-  if (!cov3D_precomp && misaligned16(rotations)) { set_last_error("gsr_scaffold_visible: rotations must be 16-byte aligned"); return -1; }
-  if ((width + TILE_X - 1) / TILE_X > 65535 || (height + TILE_Y - 1) / TILE_Y > 65535) {
-    set_last_error("gsr_scaffold_visible: image too large"); return -1;
-  }
+  const char* fn = "gsr_scaffold_visible";
+  if (N < 0 || width <= 0 || height <= 0) return fail(fn, "N >= 0, width and height > 0");
+  if (!kernel_size_ok(kernel_size)) return fail(fn, "kernel_size must be finite and >= 0");
+  if (!means3D || !viewmatrix || !projmatrix || !radii || (!cov3D_precomp && (!scales || !rotations)))
+    return fail(fn, "need means3D, the camera, radii and scales+rotations or cov3D_precomp");
+  if (!cov3D_precomp && misaligned16(rotations)) return fail(fn, "rotations must be 16-byte aligned");
+  if ((width + TILE_X - 1) / TILE_X > 65535 || (height + TILE_Y - 1) / TILE_Y > 65535) return fail(fn, "image too large");
   if (N == 0) return 0;
   ScaffoldVisArgs a{};
   a.P = N; a.W = width; a.H = height; a.means3D = means3D; a.cov3D_precomp = cov3D_precomp;
@@ -196,39 +189,39 @@ int gsr_scaffold_visible(int N, const float* means3D, const float* scales, const
   a.view = viewmatrix; a.proj = projmatrix; a.scale_modifier = scale_modifier; a.tan_fovx = tan_fovx;
   a.tan_fovy = tan_fovy; a.kernel_size = kernel_size; a.radii = radii;
   launch_scaffold_visible(a, (cudaStream_t)stream);
-  return check(cudaGetLastError(), "scaffold_visible") ? 0 : -1;
+  return launched(fn);
 }
 
 int gsr_scaffold_count(int Nv, int k, const float* opacity, int* base, int* scratch, void* stream) {
-  if (Nv < 0 || !scaffold_k_ok(k)) { set_last_error("gsr_scaffold_count: Nv >= 0 and 1 <= k <= 32"); return -1; }
-  if ((long long)Nv * k > 0x7fffffffll) { set_last_error("gsr_scaffold_count: Nv * k must fit in int32"); return -1; }
-  if (!base || (Nv > 0 && (!opacity || !scratch))) { set_last_error("gsr_scaffold_count: null pointer"); return -1; }
+  const char* fn = "gsr_scaffold_count";
+  if (Nv < 0 || !scaffold_k_ok(k)) return fail(fn, "Nv >= 0 and 1 <= k <= 32");
+  if ((long long)Nv * k > 0x7fffffffll) return fail(fn, "Nv * k must fit in int32");
+  if (!base || (Nv > 0 && (!opacity || !scratch))) return fail(fn, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  if (Nv == 0) return check(cudaMemsetAsync(base, 0, sizeof(int), st), "scaffold_count") ? 0 : -1;
+  if (Nv == 0) return check(cudaMemsetAsync(base, 0, sizeof(int), st), fn) ? 0 : -1;
   const int nb = (Nv + SCAN_THREADS - 1) / SCAN_THREADS;
   k_scaffold_count<<<nb, SCAN_THREADS, 0, st>>>(Nv, k, opacity, base, scratch);
   k_scaffold_scan_blocks<<<1, SCAN_THREADS, 0, st>>>(nb, Nv, scratch, base);
   k_scaffold_add_blocks<<<nb, SCAN_THREADS, 0, st>>>(Nv, scratch, base);
-  return check(cudaGetLastError(), "scaffold_count") ? 0 : -1;
+  return launched(fn);
 }
 
 int gsr_scaffold_decode(int Nv, int k, const int64_t* vis, const int* base, const float* anchor, const float* offset,
                         const float* scaling, const float* opacity, const float* color, const float* cov, float* xyz,
                         float* rgb, float* out_opacity, float* scales, float* rotations, void* stream) {
-  if (Nv < 0 || !scaffold_k_ok(k)) { set_last_error("gsr_scaffold_decode: Nv >= 0 and 1 <= k <= 32"); return -1; }
-  if ((long long)Nv * k > 0x7fffffffll) { set_last_error("gsr_scaffold_decode: Nv * k must fit in int32"); return -1; }
+  const char* fn = "gsr_scaffold_decode";
+  if (Nv < 0 || !scaffold_k_ok(k)) return fail(fn, "Nv >= 0 and 1 <= k <= 32");
+  if ((long long)Nv * k > 0x7fffffffll) return fail(fn, "Nv * k must fit in int32");
   if (Nv == 0) return 0;
-  if (!vis || !base || !anchor || !offset || !scaling || !opacity || !color || !cov) {
-    set_last_error("gsr_scaffold_decode: null pointer"); return -1;
-  }
-  if (misaligned16(rotations)) { set_last_error("gsr_scaffold_decode: rotations must be 16-byte aligned"); return -1; }
+  if (!vis || !base || !anchor || !offset || !scaling || !opacity || !color || !cov) return fail(fn, "null pointer");
+  if (misaligned16(rotations)) return fail(fn, "rotations must be 16-byte aligned");
   ScaffoldDecodeArgs a{};
   a.Nv = Nv; a.k = k; a.vis = reinterpret_cast<const long long*>(vis); a.base = base; a.anchor = anchor;
   a.offset = offset; a.scaling = scaling; a.opacity = opacity; a.color = color; a.cov = cov; a.xyz = xyz; a.rgb = rgb;
   a.out_opacity = out_opacity; a.scales = scales; a.rotations = rotations;
   const long long n = (long long)Nv * k;
-  k_scaffold_decode<<<(unsigned)((n + DEC_THREADS - 1) / DEC_THREADS), DEC_THREADS, 0, (cudaStream_t)stream>>>(a);
-  return check(cudaGetLastError(), "scaffold_decode") ? 0 : -1;
+  k_scaffold_decode<<<blocks(n, DEC_THREADS), DEC_THREADS, 0, (cudaStream_t)stream>>>(a);
+  return launched(fn);
 }
 
 int gsr_scaffold_decode_backward(int N, int Nv, int k, const int64_t* vis, const int* base, const float* offset,
@@ -236,23 +229,19 @@ int gsr_scaffold_decode_backward(int N, int Nv, int k, const int64_t* vis, const
                                  const float* dL_drgb, const float* dL_dopacity, const float* dL_dscales,
                                  const float* dL_drotations, float* dL_dopacity_mlp, float* dL_dcolor, float* dL_dcov,
                                  float* dL_danchor, float* dL_doffset, float* dL_dscaling, void* stream) {
-  if (N < 0 || Nv < 0 || Nv > N || !scaffold_k_ok(k)) {
-    set_last_error("gsr_scaffold_decode_backward: 0 <= Nv <= N and 1 <= k <= 32"); return -1;
-  }
-  if ((long long)N * k > 0x7fffffffll) { set_last_error("gsr_scaffold_decode_backward: N * k must fit in int32"); return -1; }
-  if (N > 0 && (!dL_danchor || !dL_doffset || !dL_dscaling)) {
-    set_last_error("gsr_scaffold_decode_backward: null pointer"); return -1;
-  }
+  const char* fn = "gsr_scaffold_decode_backward";
+  if (N < 0 || Nv < 0 || Nv > N || !scaffold_k_ok(k)) return fail(fn, "0 <= Nv <= N and 1 <= k <= 32");
+  if ((long long)N * k > 0x7fffffffll) return fail(fn, "N * k must fit in int32");
+  if (N > 0 && (!dL_danchor || !dL_doffset || !dL_dscaling)) return fail(fn, "null pointer");
   if (Nv > 0 && (!vis || !base || !offset || !scaling || !opacity || !cov || !dL_dopacity_mlp || !dL_dcolor ||
-                 !dL_dcov)) {
-    set_last_error("gsr_scaffold_decode_backward: null pointer"); return -1;
-  }
+                 !dL_dcov))
+    return fail(fn, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   if (N == 0) return 0;
   // anchors that are not visible, and dropped offsets of visible ones, get exact zeros
-  if (!check(cudaMemsetAsync(dL_danchor, 0, sizeof(float) * 3 * (size_t)N, st), "scaffold_decode_backward") ||
-      !check(cudaMemsetAsync(dL_doffset, 0, sizeof(float) * 3 * (size_t)N * k, st), "scaffold_decode_backward") ||
-      !check(cudaMemsetAsync(dL_dscaling, 0, sizeof(float) * 6 * (size_t)N, st), "scaffold_decode_backward"))
+  if (!check(cudaMemsetAsync(dL_danchor, 0, sizeof(float) * 3 * (size_t)N, st), fn) ||
+      !check(cudaMemsetAsync(dL_doffset, 0, sizeof(float) * 3 * (size_t)N * k, st), fn) ||
+      !check(cudaMemsetAsync(dL_dscaling, 0, sizeof(float) * 6 * (size_t)N, st), fn))
     return -1;
   if (Nv == 0) return 0;
   ScaffoldDecodeBwdArgs a{};
@@ -261,8 +250,8 @@ int gsr_scaffold_decode_backward(int N, int Nv, int k, const int64_t* vis, const
   a.dL_dopacity = dL_dopacity; a.dL_dscales = dL_dscales; a.dL_drotations = dL_drotations;
   a.dL_dopacity_mlp = dL_dopacity_mlp; a.dL_dcolor = dL_dcolor; a.dL_dcov = dL_dcov; a.dL_danchor = dL_danchor;
   a.dL_doffset = dL_doffset; a.dL_dscaling = dL_dscaling;
-  k_scaffold_decode_bwd<<<(Nv + DEC_THREADS - 1) / DEC_THREADS, DEC_THREADS, 0, st>>>(a);
-  return check(cudaGetLastError(), "scaffold_decode_backward") ? 0 : -1;
+  k_scaffold_decode_bwd<<<blocks(Nv, DEC_THREADS), DEC_THREADS, 0, st>>>(a);
+  return launched(fn);
 }
 
 }  // extern "C"

@@ -9,8 +9,6 @@
 #include "../../include/gsr.h"
 #include "gsr_internal.cuh"
 
-#include <string>
-
 namespace gsr {
 
 namespace {
@@ -599,20 +597,17 @@ int64_t gsr_surfel_forward(gsr_alloc_fn geometry_alloc, void* geometry_user, gsr
                            const float* projmatrix, const float* cam_pos, int prefiltered, float* out_color,
                            float* out_allmap, int* radii, int debug, void* stream) {
   (void)prefiltered;
+  const char* fn = "gsr_surfel_forward";
   if (const char* e = surfel_args_error(P, D, M, width, height, means3D, shs, colors_precomp, scales, rotations,
-                                        viewmatrix, projmatrix, cam_pos, background)) {
-    set_last_error((std::string("gsr_surfel_forward: ") + e).c_str());
-    return -1;
-  }
-  if (!geometry_alloc || !binning_alloc || !image_alloc || !out_color || !out_allmap || (P > 0 && !opacities)) {
-    set_last_error("gsr_surfel_forward: allocators, opacities, out_color and out_allmap are required");
-    return -1;
-  }
+                                        viewmatrix, projmatrix, cam_pos, background))
+    return fail(fn, e);
+  if (!geometry_alloc || !binning_alloc || !image_alloc || !out_color || !out_allmap || (P > 0 && !opacities))
+    return fail(fn, "allocators, opacities, out_color and out_allmap are required");
   const cudaStream_t st = (cudaStream_t)stream;
   const int W = width, H = height, gx = (W + TILE_X - 1) / TILE_X, gy = (H + TILE_Y - 1) / TILE_Y, T = gx * gy;
   char* gbuf = geometry_alloc(geometry_user, sgeom_bytes(P));
   char* ibuf = image_alloc(image_user, simage_bytes(W, H));
-  if (!gbuf || !ibuf) { set_last_error("gsr_surfel_forward: scratch allocation failed"); return -1; }
+  if (!gbuf || !ibuf) return fail(fn, "scratch allocation failed");
   const SurfGeom g = carve_sgeom(aligned_base(gbuf), P);
   const SurfImage si = carve_simage(aligned_base(ibuf), W, H);
   if (!check(cudaMemsetAsync(si.im.tile_count, 0, sizeof(uint32_t) * T * SUBBINS, st), "memset tile_count")) return -1;
@@ -632,7 +627,7 @@ int64_t gsr_surfel_forward(gsr_alloc_fn geometry_alloc, void* geometry_user, gsr
   if (!check(e, "read R")) return -1;
   const long long binned = (long long)counts[0];
   char* bbuf = binning_alloc(binning_user, binning_bytes(binned));
-  if (!bbuf) { set_last_error("gsr_surfel_forward: binning allocation failed"); return -1; }
+  if (!bbuf) return fail(fn, "binning allocation failed");
   const BinView b = carve_binning(aligned_base(bbuf), binned);
   if (binned > 0) {
     launch_scatter(P, gx, T, binning_view(g), si.im, b, st);
@@ -653,22 +648,16 @@ int gsr_surfel_backward(int P, int D, int M, int64_t R, const float* background,
                         float* dL_dmean3D, float* dL_dsh, float* dL_dscale, float* dL_drot, int debug, void* stream) {
   // shs == NULL: colours were precomputed (the argument check wants exactly one of shs / colors_precomp)
   static const float kAny = 0.f;
+  const char* fn = "gsr_surfel_backward";
   if (const char* e = surfel_args_error(P, D, M, width, height, means3D, shs, shs ? nullptr : &kAny, scales,
-                                        rotations, viewmatrix, projmatrix, campos, background)) {
-    set_last_error((std::string("gsr_surfel_backward: ") + e).c_str());
-    return -1;
-  }
+                                        rotations, viewmatrix, projmatrix, campos, background))
+    return fail(fn, e);
   if (P == 0) return 0;
-  if (!geom_buffer || !image_buffer || (R > 0 && !binning_buffer) || R < 0) {
-    set_last_error("gsr_surfel_backward: missing state buffers");
-    return -1;
-  }
+  if (!geom_buffer || !image_buffer || (R > 0 && !binning_buffer) || R < 0) return fail(fn, "missing state buffers");
   if (!dL_dpix || !dL_dallmap || !dL_dmean2D || !dL_dopacity || !dL_dcolor || !dL_dmean3D || !dL_dscale || !dL_drot ||
-      (shs && !dL_dsh)) {
-    set_last_error("gsr_surfel_backward: upstream gradients and every output gradient (dL_dsh with shs) are required");
-    return -1;
-  }
-  if (misaligned16(dL_drot)) { set_last_error("gsr_surfel_backward: dL_drot must be 16-byte aligned"); return -1; }
+      (shs && !dL_dsh))
+    return fail(fn, "upstream gradients and every output gradient (dL_dsh with shs) are required");
+  if (misaligned16(dL_drot)) return fail(fn, "dL_drot must be 16-byte aligned");
   const cudaStream_t st = (cudaStream_t)stream;
   const int W = width, H = height, gx = (W + TILE_X - 1) / TILE_X, gy = (H + TILE_Y - 1) / TILE_Y;
   const SurfGeom g = carve_sgeom(aligned_base(geom_buffer), P);

@@ -130,6 +130,24 @@ BWD_ALIGN = "gsr_backward: rotations, dL_drot and dL_dconic must be 16-byte alig
 NO_ACCUM = "gsr_debug_projection_backward: accum is required"
 BIG = 16 * 65535 + 1  # pixels: one tile more than a grid dimension holds
 
+_ADAM_KEEP = []  # the arrays _adam_groups hands out stay alive for the whole module
+
+
+def _adam_groups(*groups):
+    """Host address of a gsr_adam_group array: one (numel, NULL member) pair per group, every other tensor a fake
+    device address (the step reads the descriptors on the host and refuses a NULL tensor before any launch)."""
+    from gaustudio_b200.optimizers import _AdamGroup
+    arr = (_AdamGroup * len(groups))()
+    for g, (numel, null) in zip(arr, groups):
+        for i, f in enumerate(("param", "grad", "exp_avg", "exp_avg_sq")):
+            setattr(g, f, None if f == null else (1 << 20) + 4096 * i)
+        g.numel = numel
+    _ADAM_KEEP.append(arr)
+    return ctypes.addressof(arr)
+
+
+NULL_GROUP = "gsr_adam_step: null tensor in a group"
+
 # (entry point, fixed arguments, [(return value, gsr_last_error() or None, [argument overrides that trigger it]), ...]),
 # the checks in the order they fire
 CHECKS = [
@@ -186,16 +204,70 @@ CHECKS = [
          [{"geom_buffer": None}, {"accum": None}, {"geom_buffer": None, "accum": None, "P": 0}]),
         (0, None, [{"P": 0}, {"P": -2}]),
     ]),
+    ("gsr_mark_visible", {}, [
+        (0, None, [{"P": 0}, {"P": -5}]),
+        (-1, "gsr_mark_visible: null pointer", [{"means3D": None}, {"viewmatrix": None}, {"present": None}]),
+    ]),
+    ("gsr_depth2normal", {}, [
+        (0, None, [{"width": 0}, {"height": -1}]),
+        (-1, "gsr_depth2normal: null pointer", [{"depth": None}, {"out": None}, {"rot": None, "out": None}]),
+    ]),
+    ("gsr_depth2point", {}, [
+        (0, None, [{"width": -1}, {"height": 0}]),
+        (-1, "gsr_depth2point: null pointer", [{"depth": None}, {"out": None}, {"cam_to_world": None, "depth": None}]),
+    ]),
+    ("gsr_debug_export", {}, [
+        (-1, "gsr_debug_export: missing state buffers",
+         [{"geom_buffer": None}, {"image_buffer": None}, {"binning_buffer": None, "R": 5},
+          {"geom_buffer": None, "P": 0, "point_list": None}]),
+    ]),
+    ("gsr_masked_bilateral", {}, [
+        (0, None, [{"width": 0}, {"height": -1}]),
+        (-1, "gsr_masked_bilateral: d must be odd, 1..15", [{"d": 0}, {"d": 4}, {"d": 17}, {"d": -1}]),
+        (-1, "gsr_masked_bilateral: null pointer",
+         [{"d": 5, p: None} for p in ("depth", "mask", "out_depth", "out_mask", "scratch")]),
+    ]),
+    ("gsr_extract_normals", {}, [
+        (0, None, [{"width": 0}, {"height": 0}]),
+        (-1, "gsr_extract_normals: null pointer",
+         [{"filtered_depth": None}, {"fg_mask": None}, {"opacity": None}, {"median_depth": None}, {"rot": None},
+          {"neg_world_normals": None}, {"valid": None}]),
+    ]),
+    ("gsr_normal_fusion_pass", {}, [
+        (0, None, [{"n": 0}, {"n": -1}]),
+        (-1, "gsr_normal_fusion_pass: null pointer",
+         [{"n": 7, p: None} for p in ("ids", "normals", "confidences", "xyz", "sum_normals", "sum_weights")] +
+         [{"n": 7, "P": 0}]),
+    ]),
+    ("gsr_normal_fusion_mean", {}, [
+        (0, None, [{"P": 0}, {"P": -1}]),
+    ]),
+    ("gsr_knn_grid", {}, [
+        (0, None, [{"n": 0}, {"n": -3, "k": 4}]),
+        (-1, "gsr_knn_grid: null pointer",
+         [{"n": 7, "k": 4, p: None} for p in ("points", "cell_start", "grid", "out_index", "out_dist")]),
+        (-1, "gsr_knn_grid: k must be 1, 4, 8, 10 or 16", [{"n": 7, "k": 0}, {"n": 7, "k": 2}, {"n": 1, "k": 17}]),
+    ]),
+    ("gsr_adam_step", {}, [
+        (0, None, [{"n_groups": 0}, {"n_groups": -1}]),
+        (-1, "gsr_adam_step: 1..16 groups", [{"n_groups": 1, "groups": None}, {"n_groups": 17, "step": 1}]),
+        (-1, "gsr_adam_step: step counts from 1", [{"n_groups": 1, "step": 0}, {"n_groups": 16, "step": -2}]),
+        (-1, NULL_GROUP, [{"n_groups": 1, "step": 1, "groups": _adam_groups((4, m))}
+                          for m in ("param", "grad", "exp_avg", "exp_avg_sq")] +
+         [{"n_groups": 2, "step": 3, "groups": _adam_groups((0, "param"), (1, "exp_avg"))}]),
+    ]),
 ]
 
 
 @pytest.mark.parametrize("entry,fixed,checks", CHECKS,
                          ids=["forward", "forward_fused", "backward", "backward_fused", "debug_unfused", "debug_fused",
-                              "debug_accumulator"])
+                              "debug_accumulator", "mark_visible", "depth2normal", "depth2point", "debug_export",
+                              "masked_bilateral", "extract_normals", "normal_fusion_pass", "normal_fusion_mean",
+                              "knn_grid", "adam_step"])
 def test_argument_checks_fire_in_order_before_any_work(entry, fixed, checks):
-    """Each argument check of the forward, backward and projection-backward entry points returns its value and error
-    text, alone and together with the triggers of every later check, so the order in which they fire is pinned too.
-    They all fire before the library touches memory or calls CUDA, which is why this runs without a GPU."""
+    """Each argument check of the entry points listed returns its value and error text, alone and together with the
+    triggers of every later check, so the order in which they fire is pinned too.  They all fire before the library
+    touches memory or calls CUDA, which is why this runs without a GPU."""
     for k, (ret, err, variants) in enumerate(checks):
         later = {}
         for _, _, vs in reversed(checks[k + 1:]):
