@@ -62,7 +62,13 @@ __global__ void k_dilate_minmax(const float* __restrict__ depth, const unsigned 
   }
 }
 
-__device__ __forceinline__ int reflect101(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
+// OpenCV's borderInterpolate for BORDER_REFLECT_101: reflect again until the index is inside, 0 when n == 1.  One
+// reflection is not enough once the radius reaches the image size (a 1-pixel-wide map, or d = 15 on a side under 8).
+__device__ __forceinline__ int reflect101(int i, int n) {
+  if (n == 1) return 0;
+  while ((unsigned)i >= (unsigned)n) i = i < 0 ? -i : 2 * n - 2 - i;
+  return i;
+}
 
 struct SpaceKernel { float w[225]; };  // (2r+1)^2 spatial weights of the bilateral filter, 0 outside the disc
 

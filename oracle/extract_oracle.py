@@ -18,6 +18,16 @@ import numpy as np
 f32 = np.float32
 
 
+def reflect101(i, n):
+    """OpenCV's borderInterpolate for BORDER_REFLECT_101: reflect until the index is inside, 0 when n == 1."""
+    i = np.asarray(i, np.int64)
+    if n == 1:
+        return np.zeros_like(i)
+    while ((i < 0) | (i >= n)).any():
+        i = np.where(i < 0, -i, np.where(i >= n, 2 * n - 2 - i, i))
+    return i
+
+
 def masked_bilateral_filter(depth, mask, d=3, sigma_color=75.0, sigma_space=75.0):
     depth = np.asarray(depth, f32)
     mask = np.asarray(mask).astype(bool)
@@ -29,6 +39,8 @@ def masked_bilateral_filter(depth, mask, d=3, sigma_color=75.0, sigma_space=75.0
     dil = np.zeros_like(inv)
     for dy in range(-r, r + 1):
         for dx in range(-r, r + 1):
+            if abs(dy) >= H or abs(dx) >= W:  # the shifted window lies wholly outside the image
+                continue
             ys, ye = max(0, -dy), min(H, H - dy)
             xs, xe = max(0, -dx), min(W, W - dx)
             dil[ys:ye, xs:xe] |= inv[ys + dy:ye + dy, xs + dx:xe + dx]
@@ -46,7 +58,7 @@ def masked_bilateral_filter(depth, mask, d=3, sigma_color=75.0, sigma_space=75.0
     # cv2.bilateralFilter, 32F: radius = d/2, support r_ij <= radius, border REFLECT_101
     gc = -0.5 / (float(sigma_color) ** 2)
     gs = -0.5 / (float(sigma_space) ** 2)
-    pad = np.pad(norm, r, mode="reflect")
+    pad = norm[np.ix_(reflect101(np.arange(-r, H + r), H), reflect101(np.arange(-r, W + r), W))]
     num = norm.astype(np.float64).copy()
     den = np.ones((H, W), np.float64)
     if float(norm.max()) - float(norm.min()) >= np.finfo(f32).eps:  # OpenCV copies a constant image through

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+import extract_ref64 as R
 from oracle import extract_oracle as eo
 
 pytestmark = pytest.mark.gpu
@@ -28,6 +29,8 @@ def test_bilateral_matches_reference(case):
     assert m.dtype == torch.bool and torch.equal(m.cpu(), torch.from_numpy(G[f"bil_{case}_newmask"].astype(bool)))
     # tolerance: OpenCV's 4096-bin range-kernel table vs direct expf, on a ~2 unit depth range
     np.testing.assert_allclose(f.cpu().numpy(), G[f"bil_{case}_filtered"], rtol=0, atol=5e-6)
+    ref = R.bilateral64(G[f"bil_{case}_depth"], G[f"bil_{case}_mask"], int(G[f"bil_{case}_d"]), **kw)
+    R.check_bilateral(f.cpu().numpy(), m.cpu().numpy(), ref, G[f"bil_{case}_depth"])
 
 
 def test_bilateral_full_size_and_edges():
@@ -38,9 +41,8 @@ def test_bilateral_full_size_and_edges():
     opacity = torch.rand(H, W, generator=g)
     mask = opacity > 0.1
     f, m = masked_bilateral_filter(depth.to(DEV), mask.to(DEV))
-    fo, mo = eo.masked_bilateral_filter(depth.numpy(), mask.numpy())
-    assert np.array_equal(m.cpu().numpy(), mo)
-    np.testing.assert_allclose(f.cpu().numpy(), fo, rtol=0, atol=5e-6)
+    ref = R.bilateral64(depth.numpy(), mask.numpy())
+    R.check_bilateral(f.cpu().numpy(), m.cpu().numpy(), ref, depth.numpy())
     assert torch.equal(f.cpu()[~m.cpu()], depth[~m.cpu()])  # masked-out pixels keep their depth bit for bit
     # nothing valid -> pass-through; d = 1 -> identity up to the normalisation round trip
     f0, m0 = masked_bilateral_filter(depth.to(DEV), torch.zeros(H, W, dtype=torch.bool, device=DEV))
@@ -73,20 +75,23 @@ def test_extract_view_matches_oracle():
     md = pkg["rendered_median_depth"][0].cpu().numpy(); mi = pkg["rendered_median_id"][0].cpu().numpy()
     K = cam.intrinsics
     E = cam.extrinsics.cpu().numpy()
-    fo, mo = eo.masked_bilateral_filter(dp, op > np.float32(0.1))
-    assert np.array_equal(v["fg_mask"].cpu().numpy(), mo) and 0.05 < mo.mean() < 1.0
-    np.testing.assert_allclose(v["filtered_depth"].cpu().numpy(), fo, rtol=0, atol=1e-5)
+    ref = R.bilateral64(dp, op > np.float32(0.1))
+    mo = ref["new_mask"]
+    R.check_bilateral(v["filtered_depth"].cpu().numpy(), v["fg_mask"].cpu().numpy(), ref, dp)
+    assert 0.05 < mo.mean() < 1.0
     # normals stage on the SAME filtered depth (the device one), so thresholds see identical inputs
-    o = eo.view_normals(v["filtered_depth"].cpu().numpy(), mo, op, md, mi, float(K[0, 0]), float(K[1, 1]), float(K[0, 2]),
-                        float(K[1, 2]), E, radius)
-    np.testing.assert_allclose(v["cam_normals"].cpu().numpy(), o["cam_normals"], rtol=0, atol=2e-4)
+    filt = v["filtered_depth"].cpu().numpy()
+    o = eo.view_normals(filt, mo, op, md, mi, float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]), E, radius)
+    rot = np.linalg.inv(extract._extrinsics_host(cam)[:3, :3]).T.astype(np.float32)   # what extract_view uploads
+    r64 = R.view_normals64(filt, mo, op, md, float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]), rot,
+                           np.float32(radius * 0.8))
+    R.close("extract_normals: camera", v["cam_normals"].cpu().numpy(), r64["cam"], r64["A_cam"])
     valid = v["valid"].cpu().numpy()
-    edge = np.abs(o["world_sum"] + 3) < 1e-4  # sum(world) > -3 sits on a rounding edge where the fill is (-1,-1,-1)
-    assert np.array_equal(valid[~edge], o["valid"][~edge]) and valid.sum() > 100
-    both = valid & o["valid"]
-    ours = torch.zeros(valid.shape + (3,)); ours[v["valid"].cpu()] = v["normals"].cpu()
-    theirs = np.zeros(valid.shape + (3,), np.float32); theirs[o["valid"]] = o["normals"]
-    np.testing.assert_allclose(ours.numpy()[both], theirs[both], rtol=0, atol=2e-4)
+    R.exact("extract_normals: valid", valid, r64["valid"])
+    assert valid.sum() > 100
+    edge = np.abs(o["world_sum"] + 3) < 1e-4  # the oracle's float32 sum(world) > -3 may round the other way on the fill
+    assert np.array_equal(valid[~edge], o["valid"][~edge])
+    R.close("extract_normals: world", v["normals"].cpu().numpy(), r64["neg_world"][valid], r64["A_world"][valid])
     assert np.array_equal(np.sort(v["ids"].cpu().numpy()), np.sort(mi[valid].astype(np.int64)))
     assert torch.equal(v["confidences"].cpu(), torch.from_numpy(op)[v["valid"].cpu()])
 
@@ -116,9 +121,10 @@ def test_normal_fusion_passes_match_oracle():
                                    [G[f"fus_c{v}"] for v in range(V)], [G[f"fus_E{v}"][:3, 3] for v in range(V)],
                                    smooth=False)
     assert np.array_equal(uid.cpu().numpy(), ouid)
-    got = mean.cpu().numpy()
-    assert np.array_equal(np.isnan(got), np.isnan(omean))
-    np.testing.assert_allclose(np.nan_to_num(got), np.nan_to_num(omean), rtol=0, atol=1e-5)
+    ref = R.fusion64(G["fus_xyz"], [G[f"fus_ids{v}"] for v in range(V)], [G[f"fus_n{v}"] for v in range(V)],
+                     [G[f"fus_c{v}"] for v in range(V)], [G[f"fus_E{v}"][:3, 3] for v in range(V)])
+    assert np.array_equal(ref["uid"], ouid) and ref["p2"]["n_flagged"] == 0
+    R.check_mean("fusion: mean", mean.cpu().numpy(), ref["mean2"][ouid], ref["A2"][ouid])
 
 
 def test_extract_pcd_end_to_end():
@@ -169,7 +175,6 @@ def test_dense_views_fuse_like_compact_views_and_negative_ids_are_skipped():
 @pytest.mark.parametrize("n,shape", [(5000, "ball"), (40000, "shell"), (300, "line")])
 def test_device_knn_matches_ckdtree(n, shape):
     """The neighbour search of the fusion's smoothing (extract_pcd.py:170-171, scipy cKDTree there) on the device."""
-    from scipy.spatial import cKDTree
     from gaustudio_b200.extract import knn
     g = torch.Generator().manual_seed(n)
     p = torch.randn(n, 3, generator=g)
@@ -179,11 +184,10 @@ def test_device_knn_matches_ckdtree(n, shape):
         p = torch.stack([torch.linspace(0, 1, n), torch.zeros(n), torch.zeros(n)], 1) + 1e-4 * p
     p = p.float()
     dist, idx = knn(p.to(DEV), k=10)
-    rd, ri = cKDTree(p.numpy()).query(p.numpy(), k=10)
     assert torch.equal(idx[:, 0].cpu(), torch.arange(n)) and float(dist[:, 0].abs().max()) == 0.0
-    np.testing.assert_allclose(dist.cpu().numpy(), rd, rtol=1e-5, atol=1e-6)
-    same = (idx.cpu().numpy() == ri)
-    assert same.mean() > 0.999  # equal-distance neighbours may swap places
+    # every neighbour against exact float64 distances (cKDTree on float64 above 6000 points): unique, each distance
+    # within rounding, ascending, none missed
+    R.check_knn(p.numpy(), dist.cpu().numpy(), idx.cpu().numpy(), 10)
     # unusual k / tiny inputs take the exact all-pairs path
     d3, i3 = knn(p[:7].to(DEV), k=10)
     assert d3.shape == (7, 7) and torch.equal(i3[:, 0].cpu(), torch.arange(7))
