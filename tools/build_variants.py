@@ -1,7 +1,6 @@
 """Builds experiment variants of the library (extra -D flags) into gaustudio_b200/variants/libgsr_<name>.so; a variant is
-selected at run time with GSR_LIB=<path> (see tools/coresidency_ab.sh).  Test / measurement infrastructure only."""
+selected at run time with GSR_LIB=<path> (see tools/block_size_ab.sh).  Test / measurement infrastructure only."""
 import os
-import subprocess
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -27,32 +26,11 @@ VARIANTS = {
 }
 
 
-def build(names=None):
-    out_dir = os.path.join(B.HERE, "variants")
-    os.makedirs(out_dir, exist_ok=True)
+def build(names=None, force=False):
     for name, defs in VARIANTS.items():
-        if names and name not in names:
-            continue
-        lib = os.path.join(out_dir, f"libgsr_{name}.so")
-        objs, procs = [], []
-        for s in B.SOURCES:
-            o = os.path.join(out_dir, s.replace(".cu", f".{name}.o"))
-            objs.append(o)
-            procs.append((s, subprocess.Popen([B.NVCC, *B.FLAGS, *defs, "-c", os.path.join(B.CSRC, s), "-o", o],
-                                              stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
-        log = []
-        for s, p in procs:
-            out, _ = p.communicate()
-            log.append(out)
-            if p.returncode != 0:
-                sys.stderr.write(out)
-                raise RuntimeError(f"nvcc failed on {s} ({name})")
-        subprocess.check_call([B.NVCC, "-shared", "-Xlinker", f"-soname=libgsr_{name}.so", "-o", lib, *objs, "-lcudart", "-ldl"])
-        for o in objs:
-            os.remove(o)
-        open(os.path.join(out_dir, f"ptxas_{name}.log"), "w").write("\n".join(log))
-        print("built", lib)
+        if not names or name in names:
+            print(B._build(os.path.join(B.HERE, "variants", f"libgsr_{name}.so"), defs, force=force))
 
 
 if __name__ == "__main__":
-    build(sys.argv[1:])
+    build([a for a in sys.argv[1:] if a != "-f"], force="-f" in sys.argv)
