@@ -42,10 +42,11 @@ def ball(P, W, H, s0=0.05, seed=0, radius=1.0, pos=(2.2, 1.4, 1.6), opacity=None
                 campos=cam.camera_center.numpy(), tanfovx=math.tan(cam.FoVx * 0.5), tanfovy=math.tan(cam.FoVy * 0.5))
 
 
-def geom_fields(gb, P):
-    """(rect [P,2] uint32 as int64, tile_mask [P], depth [P] float32) from a geometry buffer: carve_geom's layout, every
-    array at the next 256-byte boundary (splat [P][3] float4, rect [P] uint2, cov3D [P][6], clamped [P] u8, radii,
-    tiles_touched, tile_mask [P] u32)."""
+def geom_fields(gb, P, with_splat=False):
+    """(rect [P,2] uint32 as int64, tile_mask [P], depth [P] float32, tiles_touched [P]) from a geometry buffer, and
+    with with_splat=True the whole splat record [P,12] (px, py, A, B, C, o, depth, r, g, b, index bits, tau) after them:
+    carve_geom's layout, every array at the next 256-byte boundary (splat [P][3] float4, rect [P] uint2, cov3D [P][6],
+    clamped [P] u8, radii, tiles_touched, tile_mask [P] u32)."""
     base = (-gb.data_ptr()) % 256
     offs, p = {}, base
     for name, nbytes in (("splat", 48), ("rect", 8), ("cov3D", 24), ("clamped", 1), ("radii", 4), ("touched", 4),
@@ -58,6 +59,8 @@ def geom_fields(gb, P):
     mask = view("mask", 4, torch.int32).long() & 0xffffffff
     splat = view("splat", 48, torch.float32).view(P, 12)
     touched = view("touched", 4, torch.int32).long()
+    if with_splat:
+        return rect, mask, splat[:, 6].contiguous(), touched, splat
     return rect, mask, splat[:, 6].contiguous(), touched
 
 

@@ -305,13 +305,18 @@ def check_scatter_sort(Z):
 
 
 # ---- stage: compositing ------------------------------------------------------------------------------------------------
-def check_compositing(Z):
+def check_compositing(Z, comp=None, n_contrib=True):
+    """The planes, final_T, n_contrib and median of Z's render 1 against the float64 compositing of its records.
+    comp: the comp_ref64.Compositing to compare with (default: the one of the forward's own sorted list);
+    n_contrib=False leaves n_contrib out (it counts list positions, so it is comparable on the forward's own lists
+    only).  -> comp.stats()."""
     W, H = int(Z["W"]), int(Z["H"])
     HW = W * H
-    pre = np.asarray(Z.get("in_colors_precomp", np.zeros(0)))
-    rgb = pre if pre.size else Z["r1_rgb"]
-    comp = C64.Compositing(Z["r1_means2D"], Z["r1_conic_opacity"], rgb, Z["r1_depths"], Z["r1_radii"], W, H,
-                           np.zeros(3), lists=_own_lists(Z))
+    if comp is None:
+        pre = np.asarray(Z.get("in_colors_precomp", np.zeros(0)))
+        rgb = pre if pre.size else Z["r1_rgb"]
+        comp = C64.Compositing(Z["r1_means2D"], Z["r1_conic_opacity"], rgb, Z["r1_depths"], Z["r1_radii"], W, H,
+                               np.zeros(3), lists=_own_lists(Z))
     ref = torch.zeros(5, HW, dtype=torch.float64)   # r, g, b, depth, and their common magnitude scale below
     mag = torch.zeros(5, HW, dtype=torch.float64)
     kmax = torch.zeros(HW, dtype=torch.float64)
@@ -338,10 +343,12 @@ def check_compositing(Z):
           f"tiles beyond the float64 bound (largest deviation {float(err[bad].max()):.3g})")
     bad = ok & (planes[7] != (1 - torch.as_tensor(Z["r1_final_T"]).reshape(HW)).double())
     _need("compositing", not bad.any(), lambda: f"opacity: {int(bad.sum())} pixels are not 1 - final_T")
-    nc = torch.as_tensor(Z["r1_n_contrib"].astype(np.int64)).reshape(HW)
-    bad = ok & (nc != comp.last)
-    _need("compositing", not bad.any(), lambda: f"n_contrib: {int(bad.sum())} pixels in "
-          f"{_tiles_of(bad.reshape(H, W).numpy())} tiles differ (largest deviation {int((nc - comp.last).abs()[bad].max())})")
+    if n_contrib:
+        nc = torch.as_tensor(Z["r1_n_contrib"].astype(np.int64)).reshape(HW)
+        bad = ok & (nc != comp.last)
+        _need("compositing", not bad.any(), lambda: f"n_contrib: {int(bad.sum())} pixels in "
+              f"{_tiles_of(bad.reshape(H, W).numpy())} tiles differ (largest deviation "
+              f"{int((nc - comp.last).abs()[bad].max())})")
     okm = ok & ~comp.flag_median
     has = planes[5] > 0
     bad = okm & (has != (comp.median >= 0))
