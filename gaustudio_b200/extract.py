@@ -6,18 +6,23 @@
   getNerfppNorm(cameras)                                                     gaustudio/datasets/utils.py:82-104
   extract_view(camera, render_pkg, scene_radius)                             the loop body, extract_pcd.py:314-337
   extract_pcd(renderer, pcd, cameras)                                        the loop + fusion, extract_pcd.py:309-345
+  mesh_sap(xyz, normals, res=256, sig=2)                                     `--meshing sap`, extract_pcd.py:102-106
+  dpsr(points01, normals, res, sig)                                          models/sap.py + utils/graphics_utils.py DPSR
 
 The reference moves every depth map to the host for OpenCV (dilate + bilateralFilter) and back; here the filter,
 the normal extraction and the fusion passes are CUDA kernels behind the C ABI (include/gsr.h) and nothing is
 synchronised per view.  The k-nearest-neighbour search of the final smoothing (scipy's cKDTree on the host in the
-reference) is a uniform-grid search on the device as well (`knn`, gsr_knn_grid).
+reference) is a uniform-grid search on the device as well (`knn`, gsr_knn_grid).  The Shape-as-Points meshing (DPSR
+Poisson solve + marching cubes) is CUDA kernels around torch's cuFFT (csrc/gsr_sap.cu, DESIGN.md 7h).
 """
+import ctypes as C
 import math
 
 import numpy as np
 import torch
 
-from ._lib import call, ptr
+from . import _lib
+from ._lib import ALLOC, call, ptr
 
 
 def _need_cuda(t, what):
@@ -216,3 +221,98 @@ def extract_pcd(renderer, pcd, cameras, d=3, sigma_color=75, sigma_space=75, smo
     f_dc = pcd._f_dc[unique_ids]
     rgb = SH2RGB(f_dc.reshape(f_dc.shape[0], -1)[:, :3]).clip(0, 1)
     return pcd._xyz[unique_ids], rgb, normals, views
+
+
+# ---- Shape-as-Points meshing: the `--meshing sap` step of extract_pcd.py:397-399 (models/sap.py, DPSR) ----
+_SAP_SCRATCH, _SAP_VERTICES, _SAP_FACES = 1, 2, 3  # slots of _lib.scratch
+
+
+def _sap_inputs(points, normals, res, sig, what):
+    """Refuses bad input before any device work (the device is checked last, so every other refusal also fires on CPU
+    tensors); -> (points, normals) contiguous."""
+    for t, name in ((points, what), (normals, "normals")):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"{name} must be a tensor")
+        if t.dtype != torch.float32:
+            raise ValueError(f"{name} must be float32, got {t.dtype}")
+        if t.dim() != 2 or t.shape[1] != 3:
+            raise ValueError(f"{name} must be [N,3], got {tuple(t.shape)}")
+    if points.shape != normals.shape or points.device != normals.device:
+        raise ValueError(f"{what} and normals must have the same shape and device")
+    if points.shape[0] == 0:
+        raise ValueError(f"{what} must hold at least one point")
+    if points.shape[0] > 2**31 - 1:
+        raise ValueError(f"{what} holds more than 2^31-1 points")
+    if isinstance(res, bool) or not isinstance(res, (int, np.integer)) or not 2 <= res <= 512:
+        raise ValueError(f"res must be an integer in 2..512, got {res!r}")
+    if not (isinstance(sig, (int, float, np.integer, np.floating)) and math.isfinite(sig) and sig > 0):
+        raise ValueError(f"sig must be positive and finite, got {sig!r}")
+    if not points.is_cuda:
+        raise ValueError(f"{what} and normals must be CUDA tensors (Shape-as-Points meshing has no CPU path)")
+    return points.detach().contiguous(), normals.detach().contiguous()
+
+
+def _sap_splat(points01, normals, res):
+    """point_rasterize(points01, normals, res, weighted=False) -> [3,res,res,res] float32 (no argument checks)."""
+    grid = torch.empty(3, res, res, res, dtype=torch.float32, device=points01.device)
+    with _lib.scratch(points01.device):
+        call("gsr_sap_splat", points01.device, points01.shape[0], ptr(points01), ptr(normals), int(res), ALLOC,
+             _SAP_SCRATCH, ptr(grid))
+    return grid
+
+
+def _sap_psi(points01, normals, res, sig):
+    dev = points01.device
+    grid = _sap_splat(points01, normals, res)
+    spectrum = torch.fft.rfftn(grid, dim=(1, 2, 3))  # cuFFT
+    del grid
+    phi_hat = torch.empty(res, res, res // 2 + 1, dtype=torch.complex64, device=dev)
+    call("gsr_sap_spectral", dev, int(res), float(sig), ptr(spectrum), ptr(phi_hat))
+    del spectrum
+    phi = torch.fft.irfftn(phi_hat, s=(res, res, res)).contiguous()
+    del phi_hat
+    psi = torch.empty_like(phi)
+    with _lib.scratch(dev):
+        call("gsr_sap_shift_scale", dev, points01.shape[0], ptr(points01), int(res), ptr(phi), ALLOC, _SAP_SCRATCH,
+             ptr(psi))
+    return psi
+
+
+def dpsr(points01, normals, res=256, sig=2):
+    """DPSR(res, sig, scale=True, shift=True, weighted=False) of gaustudio/utils/graphics_utils.py followed by the tanh
+    of ShapeAsPoints.generate_mesh: the grid psi [res,res,res] float32, indexed [x,y,z] with node k at k/res, positive
+    outside the shape (where the normals point) and negative inside, as the reference's.  points01 [N,3] in [0,1) and normals [N,3], float32 CUDA."""
+    p, n = _sap_inputs(points01, normals, res, sig, "points01")
+    ok = torch.stack([torch.isfinite(p).all() & torch.isfinite(n).all(), ((p >= 0) & (p < 1)).all()]).cpu()
+    if not ok[0]:
+        raise ValueError("points01 and normals must be finite")
+    if not ok[1]:
+        raise ValueError("points01 must lie in [0, 1)")
+    return _sap_psi(p, n, int(res), float(sig))
+
+
+def mesh_sap(xyz, normals, res=256, sig=2):
+    """The `--meshing sap` step of extract_pcd.py (mesh_sap -> ShapeAsPoints.from_o3d_pointcloud + generate_mesh):
+    normalise the oriented points into the unit cube, DPSR at `res` / `sig`, marching cubes of the tanh'd grid at 0,
+    and the vertices mapped back to world coordinates.  xyz, normals: [N,3] float32 CUDA, finite (drop NaN-normal rows
+    first), not all the same point.  -> (vertices [V,3] float32, faces [F,3] int64), CUDA; faces face outward."""
+    x, n = _sap_inputs(xyz, normals, res, sig, "xyz")
+    ok = torch.stack([torch.isfinite(x).all() & torch.isfinite(n).all(), (x != x[:1]).any()]).cpu()
+    if not ok[0]:
+        raise ValueError("xyz and normals must be finite")
+    if not ok[1]:
+        raise ValueError("xyz must hold at least two distinct points (their spread sets the grid's scale)")
+    dev, res = x.device, int(res)
+    points01 = torch.empty_like(x)
+    transform = torch.empty(4, dtype=torch.float32, device=dev)
+    with _lib.scratch(dev):
+        call("gsr_sap_normalize", dev, x.shape[0], ptr(x), ALLOC, _SAP_SCRATCH, ptr(points01), ptr(transform))
+    psi = _sap_psi(points01, n, res, float(sig))
+    nf = C.c_int64(0)
+    with _lib.scratch(dev) as bufs:
+        nv = call("gsr_sap_marching_cubes", dev, res, ptr(psi), ptr(transform), ALLOC, _SAP_SCRATCH, ALLOC,
+                  _SAP_VERTICES, ALLOC, _SAP_FACES, C.byref(nf))
+    F = nf.value
+    v = bufs[_SAP_VERTICES].view(torch.float32).reshape(nv, 3) if nv else torch.empty(0, 3, device=dev)
+    f = bufs[_SAP_FACES].view(torch.int64).reshape(F, 3) if F else torch.empty(0, 3, dtype=torch.int64, device=dev)
+    return v, f

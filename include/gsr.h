@@ -270,6 +270,49 @@ int gsr_mesh_texture_view(int64_t n_vertices, const float* vertices, int64_t n_f
                           const int* face_id, const float* image, int view, int* face_stamp, int* vertex_stamp,
                           int64_t* stats, float* vertex_colors, void* stream);
 
+/* ---- Shape-as-Points meshing: the `--meshing sap` step of gaustudio/scripts/extract_pcd.py (models/sap.py and the
+ * DPSR of utils/graphics_utils.py, res = 256, sig = 2, scale = shift = True, weighted = False) ----
+ * n is 1..2^31-1 and res 2..512.  Grids are float[res^3] indexed (x*res + y)*res + z, grid node k at k/res.  The FFTs
+ * between the stages are the caller's (torch.fft.rfftn / irfftn over the three grid axes).  Every sum has a fixed
+ * order: the same inputs give the same bits.  Only gsr_sap_marching_cubes synchronises with the host.
+ *
+ * xyz: device float[n*3].  Writes transform (device float[4]) = (c, s) with c = mean(xyz) and s = 1.2 max|xyz - c|
+ * over all coordinates (both reduced in double, stored as float32), and points01 (device float[n*3]) =
+ * ((xyz - c)/s + 1)/2 in float32.  scratch_alloc is asked once. */
+int gsr_sap_normalize(int64_t n, const float* xyz, gsr_alloc_fn scratch_alloc, void* scratch_user, float* points01,
+                      float* transform, void* stream);
+
+/* point_rasterize(weighted=False): grid (device float[3*res^3], one grid per normal component) = sum over points of
+ * normal * trilinear weight towards the 8 nodes around the point, cell i0 = floor(p / cs), cs = float32(1/res), node
+ * i0 + 1 wrapped to 0 at res.  points01: device float[n*3] in [0, 1) (cell indices are clamped into the grid);
+ * normals: device float[n*3].  Deterministic: points are bucketed by cell (stable in point index) and every node
+ * gathers from its 8 cells in a fixed order, summing in double.  scratch_alloc is asked once. */
+int gsr_sap_splat(int64_t n, const float* points01, const float* normals, int res, gsr_alloc_fn scratch_alloc,
+                  void* scratch_user, float* grid, void* stream);
+
+/* The spectral solve of DPSR.forward: spectrum is rfftn of the three grids, complex64 [3][res][res][res/2+1]; writes
+ * phi_hat (complex64 [res][res][res/2+1]) = -i sum_d 2 pi w_d G N_d / (-sum_d (2 pi w_d)^2 + 1e-6), 0 at w = 0, with
+ * w numpy's integer fftfreq on the first two axes and rfftfreq on the last, G = exp(-0.5 (sig 2 |w| / res)^2) formed
+ * in double and rounded to float.  sig is positive and finite. */
+int gsr_sap_spectral(int res, double sig, const float* spectrum, float* phi_hat, void* stream);
+
+/* Shift and scale: offset = mean over the points of the trilinear interpolation of phi (device float[res^3]) at
+ * points01 (the splat's weights; summed in double in a fixed order), fv0 = phi[0] - offset, and psi (device
+ * float[res^3]) = tanh(-(phi - offset) / |fv0| * 0.5).  scratch_alloc is asked once. */
+int gsr_sap_shift_scale(int64_t n, const float* points01, int res, const float* phi, gsr_alloc_fn scratch_alloc,
+                        void* scratch_user, float* psi, void* stream);
+
+/* Marching cubes of psi at 0 over the (res-1)^3 cubes of the grid, with the tables of the TSDF extraction: one vertex
+ * per crossing edge (linear zero crossing in double), faces facing psi > 0 (outside: psi is
+ * positive on the side the normals point, as in the reference).  A vertex at index coordinates q lands at
+ * (q/res * 2 - 1) * s + c with (c, s) from transform (device float[4], gsr_sap_normalize's).  Order: vertices by node
+ * then axis, faces by cube then table entry.  Reads the counts back once (blocking), then asks vertex_alloc for
+ * float[V*3] and face_alloc for int64[F*3] (not called for an empty mesh); scratch_alloc is asked once.  Returns V
+ * and writes F to *n_faces, or -1. */
+int64_t gsr_sap_marching_cubes(int res, const float* psi, const float* transform, gsr_alloc_fn scratch_alloc,
+                               void* scratch_user, gsr_alloc_fn vertex_alloc, void* vertex_user,
+                               gsr_alloc_fn face_alloc, void* face_user, int64_t* n_faces, void* stream);
+
 /* ---- optimizer step after the path (SURVEY 8f row 3) ----
  * Fused multi-tensor Adam / AdamW: replaces `torch.optim.<optimizer_name>(param_groups, **args).step()` of
  * gaustudio/pipelines/optimizers/base.py:19-30 (+ zero_grad, :32-34) for optimizer_name in {Adam, AdamW}

@@ -1,9 +1,12 @@
-"""Example: the gs-extract-pcd flow of the reference (gaustudio/scripts/extract_pcd.py) on this stack, without meshing:
+"""Example: the gs-extract-pcd flow of the reference (gaustudio/scripts/extract_pcd.py) on this stack:
     python tools/extract_pcd_example.py --model point_cloud.ply --camera cameras.json [--sh 0] [-o fused.ply]
+                                        [--meshing {sap,none}]
 Loads a 3DGS PLY and cameras.json (gaustudio_b200.io), renders every view with the vanilla renderer, runs the GPU
-post-pass (masked bilateral filter, normals, fusion) and writes the oriented surface point cloud.  With no arguments
-it runs on a synthetic scene.  Not part of the test suite (needs a GPU); every piece it calls is."""
-import argparse, sys
+post-pass (masked bilateral filter, normals, fusion) and writes the oriented surface point cloud.  With `--meshing sap`
+(the default, as in the reference) it then meshes that cloud with Shape-as-Points (extract.mesh_sap, res 256, sig 2) and
+writes fused_mesh.ply beside it.  The reference's point-cloud cleaning step is not applied.  With no model it runs on
+a synthetic scene.  Not part of the test suite (needs a GPU); every piece it calls is."""
+import argparse, os, sys
 import torch
 sys.path.insert(0, ".")
 from gaustudio_b200 import extract, io, renderers
@@ -12,6 +15,7 @@ from gaustudio_b200.synthetic import build_config
 ap = argparse.ArgumentParser()
 ap.add_argument("--model", "-m"); ap.add_argument("--camera", "-c"); ap.add_argument("--sh", type=int, default=0)
 ap.add_argument("--output", "-o", default="fused.ply")
+ap.add_argument("--meshing", choices=["sap", "none"], default="sap")
 a = ap.parse_args()
 dev = torch.device("cuda")
 if a.model:
@@ -26,3 +30,8 @@ xyz, rgb, normals, _ = extract.extract_pcd(renderer, pcd, cameras)
 keep = ~torch.isnan(normals).any(1)
 io.export_points_ply(a.output, xyz[keep], rgb[keep], normals[keep])
 print(f"{int(keep.sum())} surface points from {len(cameras)} views -> {a.output}")
+if a.meshing == "sap":
+    vertices, faces = extract.mesh_sap(xyz[keep].detach().contiguous(), normals[keep].contiguous())
+    mesh_path = os.path.join(os.path.dirname(os.path.abspath(a.output)), "fused_mesh.ply")
+    io.export_mesh_ply(mesh_path, vertices, faces)
+    print(f"{vertices.shape[0]} vertices, {faces.shape[0]} faces -> {mesh_path}")
