@@ -8,12 +8,16 @@
   extract_pcd(renderer, pcd, cameras)                                        the loop + fusion, extract_pcd.py:309-345
   mesh_sap(xyz, normals, res=256, sig=2)                                     `--meshing sap`, extract_pcd.py:102-106
   dpsr(points01, normals, res, sig)                                          models/sap.py + utils/graphics_utils.py DPSR
+  clean_point_cloud(xyz, rgb, normals)                                       extract_pcd.py:46-51
+  remove_statistical_outlier(xyz, nb_neighbors, std_ratio)                   Open3D's, called at extract_pcd.py:47
+  remove_normal_outliers(xyz, normals, nb_neighbors, angle_threshold)        extract_pcd.py:30-43
 
 The reference moves every depth map to the host for OpenCV (dilate + bilateralFilter) and back; here the filter,
 the normal extraction and the fusion passes are CUDA kernels behind the C ABI (include/gsr.h) and nothing is
 synchronised per view.  The k-nearest-neighbour search of the final smoothing (scipy's cKDTree on the host in the
 reference) is a uniform-grid search on the device as well (`knn`, gsr_knn_grid).  The Shape-as-Points meshing (DPSR
-Poisson solve + marching cubes) is CUDA kernels around torch's cuFFT (csrc/gsr_sap.cu, DESIGN.md 7h).
+Poisson solve + marching cubes) is CUDA kernels around torch's cuFFT (csrc/gsr_sap.cu, DESIGN.md 7h), and the
+point-cloud cleaning an exact k-nearest-neighbour search fused with its two consumers (csrc/gsr_clean.cu, DESIGN.md 7i).
 """
 import ctypes as C
 import math
@@ -316,3 +320,101 @@ def mesh_sap(xyz, normals, res=256, sig=2):
     v = bufs[_SAP_VERTICES].view(torch.float32).reshape(nv, 3) if nv else torch.empty(0, 3, device=dev)
     f = bufs[_SAP_FACES].view(torch.int64).reshape(F, 3) if F else torch.empty(0, 3, dtype=torch.int64, device=dev)
     return v, f
+
+
+# ---- point-cloud cleaning: clean_point_cloud of extract_pcd.py:30-51 (csrc/gsr_clean.cu, DESIGN.md 7i) ----
+_CLEAN_SCRATCH = 1  # slot of _lib.scratch
+
+
+def _clean_inputs(xyz, normals, nb_neighbors):
+    """Refuses bad input before any device work (the caller checks the device last, as _sap_inputs does).  The
+    finiteness of xyz is read back from the device together with the survivor count."""
+    for t, name in ((xyz, "xyz"), (normals, "normals")):
+        if t is None:
+            continue
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"{name} must be a tensor")
+        if t.dtype != torch.float32:
+            raise ValueError(f"{name} must be float32, got {t.dtype}")
+        if t.dim() != 2 or t.shape[1] != 3:
+            raise ValueError(f"{name} must be [N,3], got {tuple(t.shape)}")
+    if normals is not None and (normals.shape != xyz.shape or normals.device != xyz.device):
+        raise ValueError("xyz and normals must have the same shape and device")
+    if xyz.shape[0] > 2**31 - 1:
+        raise ValueError("xyz holds more than 2^31-1 points")
+    if isinstance(nb_neighbors, bool) or not isinstance(nb_neighbors, (int, np.integer)) or not 1 <= nb_neighbors <= 64:
+        raise ValueError(f"nb_neighbors must be an integer in 1..64, got {nb_neighbors!r}")
+
+
+def _on_cuda(xyz, what):
+    if not xyz.is_cuda:
+        raise ValueError(f"{what} must be CUDA tensors (point-cloud cleaning has no CPU path)")
+
+
+def _survivors(keep, xyz):
+    """Ascending int64 indices of keep != 0: one read of (count, xyz finite) sizes the compaction.  Non-finite xyz is
+    therefore refused after the pass has run on it (the kernels stay in bounds and terminate on NaN / inf), not before
+    any device work as the other refusals are."""
+    cnt, finite = torch.stack([keep.sum(dtype=torch.int64), torch.isfinite(xyz).all().long()]).tolist()
+    if not finite:
+        raise ValueError("xyz must be finite")
+    return torch.nonzero_static(keep, size=cnt).flatten()
+
+
+def remove_statistical_outlier(xyz, nb_neighbors=50, std_ratio=2.0):
+    """Open3D's PointCloud.remove_statistical_outlier(nb_neighbors, std_ratio) on xyz [N,3] float32 CUDA: the ascending
+    int64 indices of the points whose mean distance to their nb_neighbors nearest points (themselves included) is
+    > 0 and < mean + std_ratio * std over the cloud (std with Bessel's correction over N).  Raises ValueError for
+    non-finite xyz after the pass has run (the check shares the pass's one read-back)."""
+    _clean_inputs(xyz, None, nb_neighbors)
+    if not (isinstance(std_ratio, (int, float, np.integer, np.floating)) and not isinstance(std_ratio, bool)
+            and math.isfinite(std_ratio) and std_ratio > 0):
+        raise ValueError(f"std_ratio must be positive and finite, got {std_ratio!r}")
+    _on_cuda(xyz, "xyz")
+    x, dev, n = xyz.detach().contiguous(), xyz.device, xyz.shape[0]
+    if n == 0:
+        return torch.empty(0, dtype=torch.int64, device=dev)
+    avg = torch.empty(n, dtype=torch.float64, device=dev)
+    stats = torch.empty(3, dtype=torch.float64, device=dev)
+    keep = torch.empty(n, dtype=torch.uint8, device=dev)
+    with _lib.scratch(dev):
+        call("gsr_clean_statistical", dev, n, ptr(x), int(nb_neighbors), float(std_ratio), ALLOC, _CLEAN_SCRATCH,
+             ptr(avg), ptr(stats), ptr(keep))
+    return _survivors(keep, x)
+
+
+def remove_normal_outliers(xyz, normals, nb_neighbors=20, angle_threshold=math.pi / 4):
+    """remove_normal_outliers of extract_pcd.py:30-43 on xyz / normals [N,3] float32 CUDA: the ascending int64 indices of
+    the points whose mean acos(|n_i . n_j|) over their nb_neighbors - 1 nearest other points is < angle_threshold.
+    |dot| is clamped to 1 (the reference's arccos turns the float32 |n|^2 > 1 of parallel normals into NaN); NaN
+    normals are accepted and drop the points whose neighbourhood holds one.  Non-finite xyz raises ValueError after
+    the pass has run."""
+    _clean_inputs(xyz, normals, nb_neighbors)
+    if not (isinstance(angle_threshold, (int, float, np.integer, np.floating)) and not isinstance(angle_threshold, bool)
+            and math.isfinite(angle_threshold)):
+        raise ValueError(f"angle_threshold must be finite, got {angle_threshold!r}")
+    _on_cuda(xyz, "xyz and normals")
+    x, nr, dev, n = xyz.detach().contiguous(), normals.detach().contiguous(), xyz.device, xyz.shape[0]
+    if n == 0:
+        return torch.empty(0, dtype=torch.int64, device=dev)
+    mean_angle = torch.empty(n, dtype=torch.float64, device=dev)
+    keep = torch.empty(n, dtype=torch.uint8, device=dev)
+    with _lib.scratch(dev):
+        call("gsr_clean_normal", dev, n, ptr(x), ptr(nr), int(nb_neighbors), float(angle_threshold), ALLOC,
+             _CLEAN_SCRATCH, ptr(mean_angle), ptr(keep))
+    return _survivors(keep, x)
+
+
+def clean_point_cloud(xyz, rgb, normals, nb_neighbors=50, std_ratio=2.0):
+    """clean_point_cloud of extract_pcd.py:46-51: remove_statistical_outlier(nb_neighbors, std_ratio), then
+    remove_normal_outliers(20, pi/4) on its survivors.  xyz / normals [N,3] float32 CUDA, rgb [N,...] on the same
+    device.  -> (xyz, rgb, normals, index) with index the ascending int64 indices of the kept points."""
+    if not isinstance(rgb, torch.Tensor) or not isinstance(xyz, torch.Tensor) or rgb.shape[:1] != xyz.shape[:1]:
+        raise ValueError("rgb must be a tensor with one row per point")
+    _clean_inputs(xyz, normals, nb_neighbors)
+    if rgb.device != xyz.device:
+        raise ValueError("rgb must be on the device of xyz")
+    first = remove_statistical_outlier(xyz, nb_neighbors, std_ratio)
+    second = remove_normal_outliers(xyz[first].contiguous(), normals[first].contiguous(), 20, math.pi / 4)
+    index = first[second]
+    return xyz[index], rgb[index], normals[index], index

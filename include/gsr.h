@@ -313,6 +313,31 @@ int64_t gsr_sap_marching_cubes(int res, const float* psi, const float* transform
                                void* scratch_user, gsr_alloc_fn vertex_alloc, void* vertex_user,
                                gsr_alloc_fn face_alloc, void* face_user, int64_t* n_faces, void* stream);
 
+/* ---- point-cloud cleaning: clean_point_cloud of gaustudio/scripts/extract_pcd.py:30-51 (Open3D's
+ * remove_statistical_outlier, then remove_normal_outliers) ----
+ * n is 1..2^31-1 and k 1..64; xyz and normals are device float[n*3].  Neighbours are exact: squared distances are
+ * (dx dx + dy dy) + dz dz in double from the float32 coordinates, ties to the lower index.  Every sum has a fixed
+ * order: the same inputs give the same bits.  No host synchronisation; scratch_alloc is asked once per call.
+ *
+ * Test entry: the K = min(k, n) nearest points of every point, itself included, ascending; index int32[n*k] and
+ * sq_dist double[n*k] (row i, columns >= K untouched). */
+int gsr_clean_knn(int64_t n, const float* xyz, int k, gsr_alloc_fn scratch_alloc, void* scratch_user, int* index,
+                  double* sq_dist, void* stream);
+
+/* PointCloud::RemoveStatisticalOutliers(k, std_ratio): avg_dist (device double[n]) = the mean distance to the
+ * K = min(k, n) nearest points, the point itself included; stats (device double[3]) = (mean, std, threshold) with
+ * mean = sum avg / n, std = sqrt(sum_{avg > 0} (avg - mean)^2 / (n - 1)) and threshold = mean + std_ratio std;
+ * keep (device uint8[n]) = avg > 0 && avg < threshold.  std_ratio is positive and finite. */
+int gsr_clean_statistical(int64_t n, const float* xyz, int k, double std_ratio, gsr_alloc_fn scratch_alloc,
+                          void* scratch_user, double* avg_dist, double* stats, unsigned char* keep, void* stream);
+
+/* remove_normal_outliers(k, angle_threshold): mean_angle (device double[n]) = the mean over the min(k, n) - 1 nearest
+ * points other than the point itself of acos(min(|n_i . n_j|, 1)), the dot product in double (NaN when there are
+ * none, or a normal is NaN); keep (device uint8[n]) = mean_angle < angle_threshold.  angle_threshold is finite. */
+int gsr_clean_normal(int64_t n, const float* xyz, const float* normals, int k, double angle_threshold,
+                     gsr_alloc_fn scratch_alloc, void* scratch_user, double* mean_angle, unsigned char* keep,
+                     void* stream);
+
 /* ---- optimizer step after the path (SURVEY 8f row 3) ----
  * Fused multi-tensor Adam / AdamW: replaces `torch.optim.<optimizer_name>(param_groups, **args).step()` of
  * gaustudio/pipelines/optimizers/base.py:19-30 (+ zero_grad, :32-34) for optimizer_name in {Adam, AdamW}
