@@ -53,6 +53,12 @@ SIGNATURES = {
     "gsr_clean_knn": (_I, [_L, _P, _I, ALLOC_FN, _P, _P, _P, _P]),
     "gsr_clean_statistical": (_I, [_L, _P, _I, _D, ALLOC_FN, _P, _P, _P, _P, _P]),
     "gsr_clean_normal": (_I, [_L, _P, _P, _I, _D, ALLOC_FN, _P, _P, _P, _P]),
+    "gsr_dist2": (_I, [_L, _P, ALLOC_FN, _P, _P, _P]),
+    "gsr_normal2rotation": (_I, [_L, _P, _P, _P]),
+    "gsr_mesh_vertex_normals": (_I, [_L, _P, _L, _P, ALLOC_FN, _P, _P, _P]),
+    "gsr_mesh_gaussians": (_I, [_L, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "gsr_voxelize": (_L, [_L, _P, _L, _P, _I, _D, ALLOC_FN, _P, _P, _P, _P, _P, _P]),
+    "gsr_voxel_colors": (_I, [_L, _P, _P, _P, _I, _D, _P, _P, _P, _P, _P]),
     "gsr_mesh_raster_bytes": (C.c_size_t, [_L, _L, _I, _I]),
     "gsr_mesh_rasterize": (_I, [_L, _P, _L, _P, _P, _D, _D, _D, _D, _D, _I, _I, _P, C.c_size_t, _P, _P, _P]),
     "gsr_mesh_shade": (_I, [_L, _P, _L, _P, _P, _D, _D, _D, _D, _I, _I, _P, _P, _P, _P, _P, _P]),

@@ -207,11 +207,14 @@ __device__ __forceinline__ int lower_bound(const unsigned long long* __restrict_
   return lo;
 }
 
-enum { MODE_KNN = 0, MODE_STAT = 1, MODE_ANGLE = 2 };
+enum { MODE_KNN = 0, MODE_STAT = 1, MODE_ANGLE = 2, MODE_DIST2 = 3 };
 
 // MODE_KNN:   out_idx[i*k + s] / out_d2[i*k + s], s < K = min(k, n): the K nearest of point i, itself included
 // MODE_STAT:  out_val[i] = mean over those K of sqrt(d2)
 // MODE_ANGLE: out_val[i] = mean over the K = min(k, n) - 1 nearest points other than i of acos(min(|n_i . n_j|, 1))
+// MODE_DIST2: ((float*)out_val)[i] = float((d1 + d2 + d3) / 3) over the K = min(4, n) - 1 nearest points other than
+//             i (k = 4), a missing neighbour counting as +inf: distCUDA2's contract.  (The float output shares
+//             out_val so that the other modes keep their signature and code.)
 template <int MODE>
 __global__ void __launch_bounds__(KNN_THREADS, 3) k_clean_knn(int n, int k, const float4* __restrict__ sp,
                                                            const unsigned long long* __restrict__ key,
@@ -222,7 +225,8 @@ __global__ void __launch_bounds__(KNN_THREADS, 3) k_clean_knn(int n, int k, cons
   const int q = blockIdx.x * (KNN_THREADS / 32) + (threadIdx.x >> 5);
   if (q >= n) return;  // whole warps leave together
   const Lattice L = *lat;
-  const int K = MODE == MODE_ANGLE ? min(k, n) - 1 : min(k, n);
+  constexpr bool NOT_SELF = MODE == MODE_ANGLE || MODE == MODE_DIST2;
+  const int K = NOT_SELF ? min(k, n) - 1 : min(k, n);
   const float4 Q = sp[q];
   const int self = __float_as_int(Q.w);
   const double uq[3] = {lat_u(L, 0, Q.x), lat_u(L, 1, Q.y), lat_u(L, 2, Q.z)};
@@ -286,7 +290,7 @@ __global__ void __launch_bounds__(KNN_THREADS, 3) k_clean_knn(int n, int k, cons
             if (j < ce) {
               const float4 P = sp[j];
               ci = __float_as_int(P.w);
-              ok = !(MODE == MODE_ANGLE && ci == self);
+              ok = !(NOT_SELF && ci == self);
               if (ok && pl >= 0) {  // already scanned at level pl?
                 bool inside = true;
                 const float pp[3] = {P.x, P.y, P.z};
@@ -335,6 +339,15 @@ __global__ void __launch_bounds__(KNN_THREADS, 3) k_clean_knn(int n, int k, cons
         out_d2[(size_t)orig * k + s] = b.d[e];
       }
     }
+    return;
+  }
+  if (MODE == MODE_DIST2) {
+    double d[3];
+    for (int s = 0; s < 3; s++) {
+      const double ds = __shfl_sync(0xffffffffu, b.d[0], s);
+      d[s] = s < K ? ds : INFINITY;  // slots >= K may hold entries shifted past the K-th
+    }
+    if (lane == 0) reinterpret_cast<float*>(out_val)[orig] = (float)(__dadd_rn(__dadd_rn(d[0], d[1]), d[2]) / 3.0);
     return;
   }
   double v = 0.0;
@@ -514,6 +527,18 @@ int gsr_clean_normal(int64_t n, const float* xyz, const float* normals, int k, d
   k_clean_knn<MODE_ANGLE><<<knn_blocks((int)n), KNN_THREADS, 0, st>>>((int)n, k, g.sp, g.key, g.lat, normals, nullptr,
                                                                       nullptr, mean_angle);
   k_clean_keep_angle<<<blocks(n, 256), 256, 0, st>>>((int)n, mean_angle, angle_threshold, keep);
+  return launched(fn);
+}
+
+int gsr_dist2(int64_t n, const float* xyz, gsr_alloc_fn scratch_alloc, void* scratch_user, float* dist2, void* stream) {
+  const char* fn = "gsr_dist2";
+  if (!n_ok(fn, n)) return -1;
+  if (!xyz || !scratch_alloc || !dist2) return fail(fn, "xyz, scratch_alloc and dist2 are required");
+  cudaStream_t st = (cudaStream_t)stream;
+  Grid g;
+  if (!build_grid(fn, (int)n, 4, xyz, scratch_alloc, scratch_user, st, g)) return -1;
+  k_clean_knn<MODE_DIST2><<<knn_blocks((int)n), KNN_THREADS, 0, st>>>((int)n, 4, g.sp, g.key, g.lat, nullptr, nullptr,
+                                                                      nullptr, reinterpret_cast<double*>(dist2));
   return launched(fn);
 }
 

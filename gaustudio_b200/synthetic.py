@@ -60,6 +60,71 @@ class GaussianPointCloud(torch.nn.Module):
     def parameters_list(self):
         return [self._xyz, self._scale, self._rot, self._opacity, self._f_dc, self._f_rest]
 
+    @classmethod
+    def empty(cls, sh_degree=3, device="cuda"):
+        """A model with no Gaussians and active_sh_degree 0, as VanillaPointCloud.__init__ leaves it
+        (vanilla_sg.py:39-40); fill it with create_from_attribute or an initializer."""
+        z = lambda *shape: torch.zeros(*shape, dtype=torch.float32, device=device)
+        return cls(z(0, 3), z(0, 3), z(0, 4), z(0, 1), z(0, 1, 3), z(0, (sh_degree + 1) ** 2 - 1, 3), sh_degree, 0)
+
+    def create_from_attribute(self, xyz, rgb=None, scale=None, rot=None, opacity=None):
+        """vanilla_sg.py:69-97: replace the six attributes in place on the model's device.  Inputs are numpy arrays
+        or tensors, converted to float32: xyz [P,3]; rgb [P,3] in [0, 1] (None: ones) -> _f_dc = RGB2SH(rgb)
+        [P,1,3]; _f_rest zeros; scale [P,3] log-scales (None: log(sqrt(dist2(xyz) + 1e-7)) on all three axes, which
+        needs a CUDA model); rot [P,4] (None: (1, 0, 0, 0)); opacity [P,1] logits (None: inverse_sigmoid(0.1))."""
+        dev = self._xyz.device
+        host = [_float_rows(xyz, "xyz", 3)]
+        P = host[0].shape[0]
+        for a, name, w in ((rgb, "rgb", 3), (scale, "scale", 3), (rot, "rot", 4), (opacity, "opacity", 1)):
+            host.append(None if a is None else _float_rows(a, name, w, P))
+        if scale is None and dev.type != "cuda" and P > 0:
+            raise ValueError("scale=None needs dist2, which has no CPU path: move the model to a CUDA device")
+        x, rgb, scale, rot, opacity = (None if a is None else a.to(dev) for a in host)
+        if rgb is None:
+            rgb = torch.ones_like(x)
+        f_dc = ((rgb - 0.5) / SH_C0).unsqueeze(-1).transpose(1, 2).contiguous()
+        if scale is None:
+            from .initializers import dist2
+            scale = torch.log(torch.sqrt(dist2(x) + 1e-7))[..., None].repeat(1, 3)
+        if rot is None:
+            rot = torch.zeros((P, 4), dtype=torch.float32, device=dev)
+            rot[:, 0] = 1
+        if opacity is None:
+            o = 0.1 * torch.ones((P, 1), dtype=torch.float32, device=dev)
+            opacity = torch.log(o / (1 - o))
+        self._set_attributes(x, f_dc, scale, rot, opacity)
+        return self
+
+    def _set_attributes(self, xyz, f_dc, scale, rot, opacity):
+        """Replaces the six attributes.  An attribute that is an nn.Parameter (a model already set up for training)
+        becomes a new Parameter with the same requires_grad: the old one, and any optimizer state keyed on it, no
+        longer belongs to the model, so build the optimizer after (re-)initialising."""
+        P = xyz.shape[0]
+        f_rest = torch.zeros((P, (self.max_sh_degree + 1) ** 2 - 1, 3), dtype=torch.float32, device=xyz.device)
+        for k, v in zip(self._ATTRS, (xyz, scale, rot, opacity, f_dc, f_rest)):
+            old = getattr(self, k, None)
+            setattr(self, k, torch.nn.Parameter(v, requires_grad=old.requires_grad)
+                    if isinstance(old, torch.nn.Parameter) else v)
+        self.num_points = P
+
+
+SH_C0 = 0.28209479177387814  # RGB2SH of gaustudio/utils/sh_utils.py
+
+
+def _float_rows(a, name, width, rows=None):
+    """numpy array or tensor [rows, width] of real numbers -> float32 tensor on its own device (host for numpy)."""
+    if isinstance(a, np.ndarray):
+        a = torch.from_numpy(np.ascontiguousarray(a))
+    if not isinstance(a, torch.Tensor):
+        raise ValueError(f"{name} must be a numpy array or a tensor")
+    if a.dtype == torch.bool or a.is_complex() or not (a.is_floating_point() or a.dtype in
+                                                         (torch.uint8, torch.int8, torch.int16, torch.int32, torch.int64)):
+        raise ValueError(f"{name} must hold real numbers, got {a.dtype}")
+    if a.dim() != 2 or a.shape[1] != width or (rows is not None and a.shape[0] != rows):
+        want = f"[{'P' if rows is None else rows},{width}]"
+        raise ValueError(f"{name} must be {want}, got {tuple(a.shape)}")
+    return a.detach().to(torch.float32)
+
 
 def _ball(g, n, rho):
     d = torch.randn(n, 3, generator=g)

@@ -338,6 +338,48 @@ int gsr_clean_normal(int64_t n, const float* xyz, const float* normals, int k, d
                      gsr_alloc_fn scratch_alloc, void* scratch_user, double* mean_angle, unsigned char* keep,
                      void* stream);
 
+/* distCUDA2 of simple_knn (graphdeco's and gaustudio's initial scales): dist2 (device float[n]) = float of the mean of
+ * the squared distances to the 3 nearest points other than the point itself, the exact search and rounding of
+ * gsr_clean_knn, summed (d1 + d2) + d3 in double; a missing neighbour (n <= 3) counts as +inf. */
+int gsr_dist2(int64_t n, const float* xyz, gsr_alloc_fn scratch_alloc, void* scratch_user, float* dist2, void* stream);
+
+/* ---- Gaussian initialization: gaustudio/pipelines/initializers/{pcd,mesh}.py (csrc/gsr_init.cu) ----
+ * normal2rotation of pcd.py:12-37 in float32, the reference's op order: normals device float[n*3] -> rot device
+ * float[n*4] (16-byte aligned), the raw quaternion (w, x, y, z) of [R0 | R1 | normalize(n)]. */
+int gsr_normal2rotation(int64_t n, const float* normals, float* rot, void* stream);
+
+/* open3d's compute_vertex_normals: each vertex sums the face normals (v1 - v0) x (v2 - v0) of its faces in ascending
+ * face order, in double, then divides by the norm (a zero sum stays zero); normals device float[nv*3].  verts device
+ * float[nv*3], faces device int64[nf*3] with indices in [0, nv), nf < 2^31 / 3.  scratch_alloc is asked once. */
+int gsr_mesh_vertex_normals(int64_t nv, const float* verts, int64_t nf, const int64_t* faces,
+                            gsr_alloc_fn scratch_alloc, void* scratch_user, float* normals, void* stream);
+
+/* SuGaR placement of the mesh initializer (mesh.py:95-250) with n in {1, 3, 4, 6} Gaussians per face, row f n + s for
+ * slot s of face f: xyz float[3] the barycentric combination, rot float[4] (16-byte aligned) normal2rotation of the
+ * normalised interpolated vertex normal, f_dc float[3] RGB2SH of the interpolated colour (of ones when colors is NULL),
+ * scale float[3] log(2 min_edge radius_n + 1e-7) twice and log(1e-7), opacity float[1] +inf.  float32 torch ops. */
+int gsr_mesh_gaussians(int64_t nf, int n, const float* verts, const int64_t* faces, const float* vertex_normals,
+                       const float* colors, float* xyz, float* rot, float* f_dc, float* scale, float* opacity,
+                       void* stream);
+
+/* open3d's VoxelGrid::CreateFromTriangleMeshWithinBounds on [-0.5, 0.5]^3 with res (1..1024) cells per axis: cell
+ * (i, j, k), box centre (-0.5 + idx voxel_size) + voxel_size / 2 per axis and half-size voxel_size / 2, is occupied iff
+ * tribox3 (in double, its op order, a touch overlaps) passes for some triangle.  verts device double[nv*3], faces
+ * device int64[nf*3].  Reads counts back three times (blocking); asks alloc once with each of column_user, hit_user
+ * and sort_user for scratch, then with out_user for int32[2U + 1 + H]: the occupied cells' linear indices
+ * (i res + j) res + k ascending (uint32[U]), the CSR offsets (int32[U + 1]) and each cell's triangles ascending
+ * (int32[H]).  Returns U (0: nothing allocated) and writes H to *n_pairs, or -1. */
+int64_t gsr_voxelize(int64_t nv, const double* verts, int64_t nf, const int64_t* faces, int res, double voxel_size,
+                     gsr_alloc_fn alloc, void* column_user, void* hit_user, void* sort_user, void* out_user,
+                     int64_t* n_pairs, void* stream);
+
+/* Voxel colours: for each of gsr_voxelize's cells, the closest point of the mesh to its centre (squared distance in
+ * double, ties to the lower triangle), searched over the triangles of the occupied cells within +-1, and rgb
+ * (device float[ncell*3]) the barycentric interpolation there of colors (device float[nv*3]), in double. */
+int gsr_voxel_colors(int64_t ncell, const unsigned* cells, const int* offsets, const int* tris, int res,
+                     double voxel_size, const double* verts, const int64_t* faces, const float* colors, float* rgb,
+                     void* stream);
+
 /* ---- optimizer step after the path (SURVEY 8f row 3) ----
  * Fused multi-tensor Adam / AdamW: replaces `torch.optim.<optimizer_name>(param_groups, **args).step()` of
  * gaustudio/pipelines/optimizers/base.py:19-30 (+ zero_grad, :32-34) for optimizer_name in {Adam, AdamW}
