@@ -59,6 +59,9 @@ SIGNATURES = {
     "gsr_mesh_gaussians": (_I, [_L, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "gsr_voxelize": (_L, [_L, _P, _L, _P, _I, _D, ALLOC_FN, _P, _P, _P, _P, _P, _P]),
     "gsr_voxel_colors": (_I, [_L, _P, _P, _P, _I, _D, _P, _P, _P, _P, _P]),
+    "gsr_hull_carve": (_I, [_I, _D, _D, _D, _D, _I, _P, _P, _P, _P, _P]),
+    "gsr_hull_marching_cubes": (_L, [_I, _P, _D, _D, _D, _D, _D, ALLOC_FN, _P, ALLOC_FN, _P, ALLOC_FN, _P, _P,
+                                       _P]),
     "gsr_mesh_raster_bytes": (C.c_size_t, [_L, _L, _I, _I]),
     "gsr_mesh_rasterize": (_I, [_L, _P, _L, _P, _P, _D, _D, _D, _D, _D, _I, _I, _P, C.c_size_t, _P, _P, _P]),
     "gsr_mesh_shade": (_I, [_L, _P, _L, _P, _P, _D, _D, _D, _D, _I, _I, _P, _P, _P, _P, _P, _P]),

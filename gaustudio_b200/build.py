@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SOURCES = ["gsr_api.cu", "gsr_preprocess.cu", "gsr_binning.cu", "gsr_render.cu", "gsr_extract.cu", "gsr_mesh.cu",
            "gsr_meshraster.cu", "gsr_surfel.cu", "gsr_mip.cu", "gsr_scaffold.cu", "gsr_densify.cu",
-           "gsr_loss.cu", "gsr_adam.cu", "gsr_sap.cu", "gsr_clean.cu", "gsr_init.cu"]
+           "gsr_loss.cu", "gsr_adam.cu", "gsr_sap.cu", "gsr_clean.cu", "gsr_init.cu", "gsr_hull.cu"]
 LIB = os.path.join(HERE, "libgsr_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",

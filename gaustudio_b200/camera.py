@@ -6,7 +6,9 @@ Mirrors the fields and numerics of the reference dataclass
 `intrinsics` / `extrinsics` properties (`:219-237`), so that
 `BaseRenderer.render(camera, model)` (`gaustudio/renderers/base.py:10-63`) reads
 identical `world_view_transform`, `full_proj_transform`, `camera_center`,
-`FoVx`, `FoVy`, `image_width`, `image_height`.  No image / dataset I/O (out of scope).
+`FoVx`, `FoVy`, `image_width`, `image_height`.  The per-view `image`, `mask` and `depth` fields (`:139-143`) and
+their resizes (`downsample`, `:246-266`) are there for the initializers that read posed views; loading them from disk
+(the dataset loaders) is out of scope.
 """
 import dataclasses
 import math
@@ -67,6 +69,9 @@ class Camera:
     projection_matrix: torch.Tensor = None
     camera_center: torch.Tensor = None
     principal_point_ndc: np.ndarray = None
+    image: torch.Tensor = None  # [H,W,3] float in [0, 1]
+    mask: torch.Tensor = None   # [H,W], nonzero = foreground
+    depth: torch.Tensor = None  # [H,W] float32
 
     def __post_init__(self):
         self._setup()
@@ -103,9 +108,37 @@ class Camera:
                              [0, fy, self.image_height * self.principal_point_ndc[1]],
                              [0, 0, 1]]).float()
 
-    def depth2point(self, depth, coordinate="camera"):
-        """[H,W] depth -> [H,W,3] points (CUDA restatement of datasets/__init__.py:307-339)."""
+    @property
+    def fx(self):
+        return self.intrinsics[0, 0]
+
+    @property
+    def fy(self):
+        return self.intrinsics[1, 1]
+
+    def downsample_scale(self, scale):
+        """downsample to (round(W / scale), round(H / scale)) (datasets/__init__.py:246-249)."""
+        return self.downsample((round(self.image_width / scale), round(self.image_height / scale)))
+
+    def downsample(self, resolution):
+        """Resize image, mask and depth to resolution = (W, H) with PIL, as the reference does (:251-266): image and
+        mask through resize_image, depth through resize_depth.  Replaces the fields (host tensors) and the size."""
+        if self.image is not None:
+            self.image = resize_image(self.image, resolution)[..., :3].clamp(0.0, 1.0)
+        if self.mask is not None:
+            self.mask = resize_image(self.mask, resolution).clamp(0.0, 1.0)
+        if self.depth is not None:
+            self.depth = resize_depth(self.depth, resolution)
+        self.image_width, self.image_height = resolution
+        return self
+
+    def depth2point(self, depth=None, coordinate="camera"):
+        """[H,W] depth (default: self.depth) -> [H,W,3] points (CUDA restatement of datasets/__init__.py:307-339)."""
         from . import ops
+        if depth is None:
+            depth = self.depth
+        if depth is None:
+            raise ValueError("Depth is not available.")
         K = self.intrinsics
         c2w = torch.inverse(self.extrinsics) if coordinate == "world" else None
         return ops.depth2point(depth, float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]), c2w)
@@ -119,6 +152,31 @@ class Camera:
             rot = self.extrinsics[:3, :3].inverse().t().contiguous().to(depth.device)
         return ops.depth2normal(depth, float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]),
                                 d_min, d_max, rot)
+
+
+def _host(t):
+    return t.detach().cpu() if isinstance(t, torch.Tensor) else torch.from_numpy(np.asarray(t))
+
+
+def resize_image(image, resolution):
+    """resizeTorch (datasets/__init__.py:10-24): values scaled by 255 when the maximum is <= 1, truncated to uint8,
+    resized by PIL's Image.resize with its default resample, -> float32 / 255 on the host."""
+    from PIL import Image
+    t = _host(image)
+    if t.max() <= 1.0:
+        t = t * 255.0
+    pil = Image.fromarray(t.byte().numpy())
+    return torch.from_numpy(np.array(pil.resize(resolution))).float() / 255.0
+
+
+def resize_depth(depth, resolution):
+    """resizeDepthTorch (datasets/__init__.py:26-43): PIL mode F, NEAREST -> float32 [H,W] on the host."""
+    from PIL import Image
+    t = _host(depth)
+    if t.dim() != 2:
+        raise ValueError("Input tensor must have shape [H, W]")
+    pil = Image.fromarray(t.numpy().astype(np.float32))
+    return torch.from_numpy(np.array(pil.resize(resolution, Image.NEAREST)).astype(np.float32))
 
 
 def look_at_camera(position, target, W, H, FoVx, FoVy, up=(0.0, 0.0, 1.0), **kw):

@@ -1,20 +1,26 @@
-"""Gaussian initialization on the GPU: the initializers of gaustudio/pipelines/initializers/ that need no dataset
-loader, behind the reference's registry surface (`initializers/__init__.py:10-24`).
+"""Gaussian initialization on the GPU: the initializers of gaustudio/pipelines/initializers/ that need no external
+tool, behind the reference's registry surface (`initializers/__init__.py:10-24`).
 
   dist2(xyz)                         distCUDA2 of simple_knn: mean squared distance to the 3 nearest other points
   normal2rotation(normals)           pcd.py:12-37 (the raw quaternion of [R0 | R1 | n])
   make({"name": "pcd", "model_path": ...})           pcd.py:39-77
   make({"name": "mesh", "n_gaussians_per_surface_triangle": n})   mesh.py:74-250 (SuGaR placement)
   make({"name": "voxel", "voxel_size": s})           mesh.py:252-442
+  make({"name": "VisualHull", "resolution": 128, ...})   mask.py:16-108 (space carving against the views' masks)
+  make({"name": "depth", "workspace_dir": ...})        depth.py:18-91 (back-projected depth maps)
 
-An initializer is called as the reference calls it, `init(model, mesh=None, dataset=None, overwrite=False)`; it fills
-`model` (a GaussianPointCloud) through `create_from_attribute` and returns it.  The kernels are in csrc/gsr_init.cu
-and csrc/gsr_clean.cu (MODE_DIST2); DESIGN.md 7j states the contract and the departures from the reference.
+An initializer is called as the reference calls it: `init(model, mesh=None, dataset=None, overwrite=False)` for the
+mesh-based ones, `init(model, dataset, overwrite=False)` for VisualHull and depth, whose dataset is an iterable of
+cameras carrying masks or depth maps.  It fills `model` (a GaussianPointCloud) through `create_from_attribute` and
+returns it.  The kernels are in csrc/gsr_init.cu, csrc/gsr_clean.cu (MODE_DIST2) and csrc/gsr_hull.cu; DESIGN.md 7j
+and 7k state the contracts and the departures from the reference.
 """
 from collections.abc import Mapping
+import copy
 import ctypes as C
 import math
 import os
+import tempfile
 
 import numpy as np
 import torch
@@ -299,3 +305,227 @@ def voxelize(vertices, faces, res, voxel_size):
                 torch.empty(0, dtype=torch.int32, device=dev))
     out = bufs[_VOX_OUT].view(torch.int32)
     return out[:U], out[U:2 * U + 1], out[2 * U + 1:2 * U + 1 + H]
+
+
+# ---- VisualHull (mask.py) and depth (depth.py): initializers that read posed views (csrc/gsr_hull.cu, DESIGN.md 7k) --
+_HULL_VERTICES, _HULL_FACES = 2, 3
+MAX_HULL_RES = 512  # the marching cubes' limit
+
+
+def _workspace(config):
+    ws = config.get("workspace_dir")
+    if ws is None:
+        ws = tempfile.mkdtemp()
+    os.makedirs(ws, exist_ok=True)
+    return ws
+
+
+def scene_extent(dataset, cameras):
+    """-> (translate [3] float64, min_extent): the dataset's `cameras_center` / `cameras_min_extent` when it has them,
+    else getNerfppNorm's `translate` / `min_radius` of the cameras (the values the reference's loaders store there)."""
+    if hasattr(dataset, "cameras_center") and hasattr(dataset, "cameras_min_extent"):
+        t = dataset.cameras_center
+        t = t.detach().cpu().numpy() if isinstance(t, torch.Tensor) else t
+        return np.asarray(t, np.float64).reshape(3), float(dataset.cameras_min_extent)
+    from .extract import getNerfppNorm
+    norm = getNerfppNorm(cameras)
+    return np.asarray(norm["translate"], np.float64).reshape(3), float(norm["min_radius"])
+
+
+def _check_views(cameras):
+    for cam in cameras:
+        W, H = int(cam.image_width), int(cam.image_height)
+        if W < 1 or H < 1:
+            raise ValueError(f"camera size must be positive, got {W}x{H}")
+        m = getattr(cam, "mask", None)
+        if m is not None and tuple(m.shape) != (H, W):
+            raise ValueError(f"a mask must have the camera's shape [H,W] = [{H},{W}], got {list(m.shape)}")
+
+
+def _hull_views(cameras, dev):
+    """Camera records of gsr_hull_carve on dev: (proj float32 [C,16], views int64 [C,3], masks uint8 [sum H W])."""
+    proj, views, masks, off = [], [], [], 0
+    for cam in cameras:
+        W, H = int(cam.image_width), int(cam.image_height)
+        m = getattr(cam, "mask", None)
+        if m is not None:
+            masks.append(m)
+        views.append((W, H, off if m is not None else -1))
+        off += H * W if m is not None else 0
+        proj.append(torch.as_tensor(cam.full_proj_transform).detach().float().cpu().reshape(16))
+    P = torch.stack(proj).to(dev) if proj else torch.empty(0, 16, device=dev)
+    V = torch.tensor(views, dtype=torch.int64).reshape(-1, 3).to(dev)
+    M = torch.cat([(torch.as_tensor(m).to(dev) != 0).to(torch.uint8).reshape(-1) for m in masks]) if masks else None
+    return P.contiguous(), V.contiguous(), M
+
+
+def _hull_args(res, radius, translate):
+    if isinstance(res, bool) or not isinstance(res, (int, np.integer)) or not 2 <= int(res) <= MAX_HULL_RES:
+        raise ValueError(f"resolution must be an integer in 2..{MAX_HULL_RES}, got {res!r}")
+    if not (math.isfinite(radius) and radius > 0):
+        raise ValueError(f"the carving radius must be positive and finite, got {radius!r} (one camera, or cameras "
+                         "at one point, give 0)")
+    t = np.asarray(translate, np.float64).reshape(3)
+    if not np.isfinite(t).all():
+        raise ValueError("translate must be finite")
+    return int(res), float(radius), t
+
+
+def visual_hull_carve(cameras, res, radius, translate, device="cuda"):
+    """The carving of mask.py:38-69: occupancy uint8 [res,res,res] (the reference's `volume`) of the nodes
+    np.meshgrid(lin, lin, lin) - translate, lin = np.linspace(-radius, radius, res), that pass every camera's
+    insideView against its mask (no mask: the view frustum alone).  One kernel; DESIGN.md 7k."""
+    res, radius, t = _hull_args(res, radius, translate)
+    cameras = list(cameras)
+    _check_views(cameras)
+    dev = torch.device(device)
+    if dev.type != "cuda":
+        raise ValueError("the visual hull has no CPU path: use a CUDA device")
+    P, V, M = _hull_views(cameras, dev)
+    occ = torch.empty(res, res, res, dtype=torch.uint8, device=dev)
+    call("gsr_hull_carve", dev, res, radius, *map(float, t), len(cameras), ptr(P), ptr(V), ptr(M), ptr(occ))
+    return occ
+
+
+def visual_hull_mesh(occ, threshold, radius, translate):
+    """extract_mesh of mask.py:82-93 on a carved occupancy: marching cubes at `threshold`, vertices mapped to the world
+    -> (vertices [V,3] float32, faces [F,3] int64) on occ's device, faces facing the carved side."""
+    if not (isinstance(occ, torch.Tensor) and occ.is_cuda and occ.dtype == torch.uint8 and occ.dim() == 3
+            and occ.shape[0] == occ.shape[1] == occ.shape[2]):
+        raise ValueError("occ must be a cubic uint8 CUDA tensor [res,res,res]")
+    res, radius, t = _hull_args(occ.shape[0], radius, translate)
+    if not 0.0 < threshold < 1.0:
+        raise ValueError(f"threshold must be in (0, 1), got {threshold!r}")
+    dev, occ = occ.device, occ.contiguous()
+    nf = C.c_int64(0)
+    with _lib.scratch(dev) as bufs:
+        nv = call("gsr_hull_marching_cubes", dev, res, ptr(occ), float(threshold), radius, *map(float, t), ALLOC,
+                  _SCRATCH, ALLOC, _HULL_VERTICES, ALLOC, _HULL_FACES, C.byref(nf))
+    F = nf.value
+    v = bufs[_HULL_VERTICES].view(torch.float32).reshape(nv, 3) if nv else torch.empty(0, 3, device=dev)
+    f = bufs[_HULL_FACES].view(torch.int64).reshape(F, 3) if F else torch.empty(0, 3, dtype=torch.int64, device=dev)
+    return v, f
+
+
+@register("VisualHull")
+class VisualHullInitializer(BaseInitializer):
+    """mask.py:16-108: carve a `resolution`^3 grid of half-width r = cameras_min_extent * radius_scale around the
+    scene centre against every camera's mask, mesh the occupancy at `threshold` into `workspace_dir`/visual_hull.ply,
+    and put one Gaussian on each mesh vertex with the reference's constants: rgb 0.5, opacity logit 0.1, log-scale 0.01
+    (passed to create_from_attribute unchanged).  Returns the model (the reference returns None)."""
+
+    def __init__(self, config):
+        super().__init__(config)
+        cfg = self.initializer_config
+        res, th, rs = cfg.get("resolution", 128), cfg.get("threshold", 0.5), cfg.get("radius_scale", 1.2)
+        if isinstance(res, bool) or not isinstance(res, (int, np.integer)) or not 2 <= int(res) <= MAX_HULL_RES:
+            raise ValueError(f"resolution must be an integer in 2..{MAX_HULL_RES}, got {res!r}")
+        if isinstance(th, bool) or not isinstance(th, (int, float, np.integer, np.floating)) or not 0.0 < th < 1.0:
+            raise ValueError(f"threshold must be in (0, 1), got {th!r}")
+        if isinstance(rs, bool) or not isinstance(rs, (int, float, np.integer, np.floating)) or \
+                not math.isfinite(rs):
+            raise ValueError(f"radius_scale must be a finite number, got {rs!r}")
+        self.resolution, self.threshold, self.radius_scale = int(res), float(th), float(rs)
+        self.ws_dir = _workspace(cfg)
+
+    def __call__(self, model, dataset, overwrite=False):
+        if overwrite or not os.path.exists(os.path.join(self.ws_dir, "visual_hull.ply")):
+            self.construct_visual_hull(dataset, _device_of(model))
+        return self.build_model(model)
+
+    def construct_visual_hull(self, dataset, device="cuda"):
+        cameras = list(dataset)
+        if not cameras:
+            raise ValueError("the dataset has no cameras")
+        translate, extent = scene_extent(dataset, cameras)
+        radius = extent * self.radius_scale
+        occ = visual_hull_carve(cameras, self.resolution, radius, translate, device)
+        if not bool(occ.any()):
+            raise ValueError("the visual hull is empty: no grid node is inside every camera's mask")
+        v, f = visual_hull_mesh(occ, self.threshold, radius, translate)
+        if v.shape[0] == 0:
+            raise ValueError("the visual hull has no surface: every grid node is inside every camera's mask")
+        from .io import export_mesh_ply
+        export_mesh_ply(os.path.join(self.ws_dir, "visual_hull.ply"), v, f)
+        return v, f
+
+    def build_model(self, model):
+        from .io import load_mesh_ply
+        dev = _device_of(model)
+        xyz = load_mesh_ply(os.path.join(self.ws_dir, "visual_hull.ply"))[0].to(dev)
+        P = xyz.shape[0]
+        ones = lambda w: torch.ones((P, w), dtype=torch.float32, device=dev)
+        model.create_from_attribute(xyz=xyz, rgb=ones(3) * 0.5, opacity=ones(1) * 0.1, scale=ones(3) * 0.01)
+        return model
+
+
+@register("depth")
+class DepthInitializer(BaseInitializer):
+    """depth.py:18-91: every view with a depth map, downsampled by 4, back-projected to world points (one row per
+    pixel, depth 0 included), coloured by its image, scale depth / ((fx + fy) / 2); the reference's float16 round trip
+    through `fused.ply` (double x y z of the float16 points, uchar colours trunc(float16(rgb16 * 255))) and
+    `scales.bin` (raw float16) is kept exactly.  The model gets rgb = colour / 255, log-scale numpy's float16
+    log(scale16) on all three axes (-inf where the depth is 0, as in the reference) and opacity logit 0.  When fused.ply exists and
+    overwrite is False the model is built from the workspace; without scales.bin the scales come from dist2."""
+
+    def __init__(self, config):
+        super().__init__(config)
+        self.ws_dir = _workspace(self.initializer_config)
+
+    def __call__(self, model, dataset, overwrite=False):
+        if overwrite or not os.path.exists(os.path.join(self.ws_dir, "fused.ply")):
+            self.process_dataset(dataset, _device_of(model))
+        return self.build_model(model)
+
+    @staticmethod
+    def prepare_views(dataset):
+        """Copies of the cameras with a depth map, downsampled by 4 on the host; the caller's cameras are untouched."""
+        views = []
+        for cam in dataset:
+            if cam.depth is None:
+                continue
+            if cam.image is None or cam.image.dim() != 3 or tuple(cam.image.shape[:2]) != tuple(cam.depth.shape):
+                raise ValueError("a view with a depth map needs an image [H,W,3] of the same size, got "
+                                 f"{None if cam.image is None else list(cam.image.shape)} for depth "
+                                 f"{list(cam.depth.shape)}")
+            views.append(copy.copy(cam).downsample_scale(4))
+        if not views:
+            raise ValueError("no camera has a depth map")
+        return views
+
+    def process_dataset(self, dataset, device="cuda"):
+        """-> (xyz16 [N,3], colors uint8 [N,3], scale16 [N,1]) on device, also written to the workspace."""
+        from .io import export_points_ply
+        views = self.prepare_views(dataset)
+        dev = torch.device(device)
+        if dev.type != "cuda":
+            raise ValueError("the depth initializer back-projects on the device: use a CUDA model")
+        xyz, rgb, scale = [], [], []
+        for cam in views:
+            depth = cam.depth.to(dev, torch.float32).contiguous()
+            xyz.append(cam.depth2point(depth, coordinate="world").reshape(-1, 3))
+            rgb.append(cam.image.to(dev, torch.float32).reshape(-1, 3))
+            scale.append((depth / ((cam.fx + cam.fy) / 2)).reshape(-1, 1))
+        xyz16, rgb16, scale16 = (torch.cat(a).half() for a in (xyz, rgb, scale))
+        colors = (rgb16 * 255).to(torch.uint8)
+        export_points_ply(os.path.join(self.ws_dir, "fused.ply"), xyz16.double(), colors)
+        scale16.cpu().numpy().tofile(os.path.join(self.ws_dir, "scales.bin"))
+        return xyz16, colors, scale16
+
+    def build_model(self, model):
+        from .io import read_ply_vertices
+        dev = _device_of(model)
+        v = read_ply_vertices(os.path.join(self.ws_dir, "fused.ply"))
+        xyz = torch.from_numpy(np.stack([v[k] for k in "xyz"], 1).astype(np.float32)).to(dev)
+        colors = torch.from_numpy(np.stack([v[k] for k in ("red", "green", "blue")], 1).astype(np.uint8)).to(dev)
+        rgb = colors.float() / 255.0
+        log_scales = None
+        path = os.path.join(self.ws_dir, "scales.bin")
+        if os.path.exists(path):
+            # numpy's float16 log, as the reference takes it: it is not float32 log rounded to float16 (numpy 2.3 on
+            # x86-64 differs from that in 13265 of the 31743 positive finite float16 values), so it stays on the host
+            log16 = np.log(np.fromfile(path, dtype=np.float16).reshape(-1, 1))
+            log_scales = torch.from_numpy(log16).to(dev).repeat(1, 3).float()
+        opacity = torch.zeros((xyz.shape[0], 1), dtype=torch.float32, device=dev)  # inverse_sigmoid(0.5)
+        model.create_from_attribute(xyz=xyz, rgb=rgb, opacity=opacity, scale=log_scales)
+        return model

@@ -187,7 +187,7 @@ def export_scaffold(model, ply_path):
 def export_points_ply(path, xyz, rgb=None, normals=None):
     """Surface point cloud (the `fused.ply` of gaustudio/scripts/extract_pcd.py:339-352, written there through
     open3d's `write_point_cloud`): binary little-endian, double x y z [nx ny nz] + uchar red green blue, the property
-    layout open3d emits.  Tensors or arrays; colours in [0, 1]."""
+    layout open3d emits.  Tensors or arrays; colours in [0, 1], or uint8 colours written as they are."""
     def host(a):
         return None if a is None else np.asarray(a.detach().cpu() if isinstance(a, torch.Tensor) else a)
     xyz, rgb, normals = host(xyz), host(rgb), host(normals)
@@ -204,7 +204,8 @@ def export_points_ply(path, xyz, rgb=None, normals=None):
         for i, k in enumerate(("nx", "ny", "nz")):
             rec[k] = normals[:, i]
     if rgb is not None:
-        c = np.clip(np.nan_to_num(rgb.astype(np.float64)) * 255.0, 0, 255).astype(np.uint8)  # open3d truncates
+        c = rgb if rgb.dtype == np.uint8 else \
+            np.clip(np.nan_to_num(rgb.astype(np.float64)) * 255.0, 0, 255).astype(np.uint8)  # open3d truncates
         for i, k in enumerate(("red", "green", "blue")):
             rec[k] = c[:, i]
     names = {"<f8": "double", "u1": "uchar"}

@@ -380,6 +380,32 @@ int gsr_voxel_colors(int64_t ncell, const unsigned* cells, const int* offsets, c
                      double voxel_size, const double* verts, const int64_t* faces, const float* colors, float* rgb,
                      void* stream);
 
+/* ---- VisualHull: space carving of gaustudio/pipelines/initializers/mask.py (csrc/gsr_hull.cu) ----
+ * res is 2..512, radius r > 0 and (tx, ty, tz) the reference's `translate`, all finite.  The grid has res^3 nodes,
+ * node g = (i res + j) res + k at float32(lin[j] - tx, lin[i] - ty, lin[k] - tz) with lin = np.linspace(-r, r, res)
+ * (i step + start in double, no contraction, the last node exactly r): the reference's meshgrid order.
+ *
+ * Carve: occ (device uint8[res^3]) = 1 iff the node passes the reference's Camera.insideView for every camera, in
+ * order, evaluated in double from the float32 node and the float32 full_proj_transform P (device float[n_cams*16],
+ * row-major as stored): clip = [x y z 1] P summed in row order, clip_z > 0, ndc = clip_xy / clip_w in [-1, 1]^2 (inf
+ * and NaN fail), px = min(trunc((ndc_x + 1) 0.5 W), W - 1), py likewise with H, and mask[py][px] != 0.  views (device
+ * int64[n_cams*3]) = (W, H, offset of the camera's [H][W] mask in masks, or -1: no mask, every pixel inside); masks
+ * is device uint8.  n_cams = 0 fills every node.  No atomics. */
+int gsr_hull_carve(int res, double radius, double tx, double ty, double tz, int n_cams, const float* proj,
+                   const int64_t* views, const unsigned char* masks, unsigned char* occ, void* stream);
+
+/* Marching cubes of occ (gsr_hull_carve's) at threshold in (0, 1): mcubes.marching_cubes(volume, threshold) with the
+ * reference's fliplr and axis swap.  One vertex per grid edge whose ends differ, at index coordinate q = c + threshold
+ * from an empty node c, c + (1 - threshold) from a filled one (double), mapped to the world per axis as
+ * ((q / (res - 1)) (2 r) - r) - t in double and rounded once; world x comes from the grid's j axis and y from its i
+ * axis.  Faces face the empty side.  Order: vertices by node then axis (i, j, k), faces by cube then table entry.  Reads
+ * the counts back once (blocking), then asks vertex_alloc for float[V*3] and face_alloc for int64[F*3] (not called for
+ * an empty mesh); scratch_alloc is asked once.  Returns V and writes F to *n_faces, or -1. */
+int64_t gsr_hull_marching_cubes(int res, const unsigned char* occ, double threshold, double radius, double tx,
+                                double ty, double tz, gsr_alloc_fn scratch_alloc, void* scratch_user,
+                                gsr_alloc_fn vertex_alloc, void* vertex_user, gsr_alloc_fn face_alloc, void* face_user,
+                                int64_t* n_faces, void* stream);
+
 /* ---- optimizer step after the path (SURVEY 8f row 3) ----
  * Fused multi-tensor Adam / AdamW: replaces `torch.optim.<optimizer_name>(param_groups, **args).step()` of
  * gaustudio/pipelines/optimizers/base.py:19-30 (+ zero_grad, :32-34) for optimizer_name in {Adam, AdamW}
