@@ -309,6 +309,19 @@ def rasterize_gaussians_fused_backward(background, means3D, radii, f_dc, f_rest,
     return d_m2, d_op, d_m3, d_dc, d_rest, d_sc, d_rot
 
 
+def contribution(P, image_height, image_width, geomBuffer, R, binningBuffer, imageBuffer, weight, count, max_weight):
+    """Adds one view's contribution statistics (gsr_contribution) into weight float64[P], count int64[P] and
+    max_weight float32[P] (contiguous, on the buffers' device).  The buffers and R are those a rasterize_gaussians,
+    its fused variant or rasterize_gaussians_mip returned for that view.  No host synchronisation."""
+    dev = geomBuffer.device
+    for t, dt, name in ((weight, torch.float64, "weight"), (count, torch.int64, "count"),
+                        (max_weight, torch.float32, "max_weight")):
+        if t.dtype != dt or tuple(t.shape) != (P,) or t.device != dev or not t.is_contiguous():
+            raise ValueError(f"contribution: {name} must be a contiguous {dt} tensor of shape ({P},) on {dev}")
+    call("gsr_contribution", dev, int(P), int(R), int(image_width), int(image_height), _ptr(geomBuffer),
+         _ptr(binningBuffer), _ptr(imageBuffer), _ptr(weight), _ptr(count), _ptr(max_weight))
+
+
 # ---- Mip-Splatting: gsr_forward_mip / gsr_backward_mip / gsr_mip_filter3d (include/gsr.h) -----------------------------
 def _check_kernel_size(kernel_size):
     k = float(kernel_size)

@@ -27,6 +27,7 @@ SIGNATURES = {
                          _P, _P, _P, _P, _F, _F, _I, _P, _P, _P, _P, _P, _I, _L, _P, _P]),
     "gsr_backward": (_I, [_I, _I, _I, _L, _P, _I, _I, _P, _P, _P, _P, _F, _P, _P, _P, _P, _P, _F, _F, _P, _P, _P, _P,
                           _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P]),
+    "gsr_contribution": (_I, [_I, _L, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     "gsr_forward_fused": (_L, [ALLOC_FN, _P, ALLOC_FN, _P, ALLOC_FN, _P, _I, _I, _I, _P, _I, _I, _P, _P, _P, _P, _P, _F, _P,
                                _P, _P, _P, _F, _F, _I, _P, _P, _P, _P, _P, _I, _L, _P, _P]),
     "gsr_backward_fused": (_I, [_I, _I, _I, _L, _P, _I, _I, _P, _P, _P, _P, _P, _F, _P, _P, _P, _P, _F, _F, _P, _P, _P,

@@ -28,6 +28,7 @@
 //    accumulated as raw moments of u = dL/dG * G (sum u dx, u dy, u dx^2, u dx dy, u dy^2) that the
 //    per-Gaussian kernel turns into dL/dmean2D and dL/dconic.  Traversal starts at the tile's largest
 //    n_contrib instead of the end of the list.
+#include "../../include/gsr.h"
 #include "gsr_internal.cuh"
 #include <cstdlib>
 #include <cstring>
@@ -99,6 +100,19 @@ __device__ __forceinline__ void stage_gather_tma(float4* dst, const float4* __re
   const int mine = cnt > lane ? (cnt - lane + 31) / 32 : 0;
   mbar_arrive_expect(full, (unsigned)(mine * SPLAT_BYTES));
   for (int r = lane; r < cnt; r += 32) tma_copy(dst + r * SPLAT_F4, splat + (size_t)ids[r] * SPLAT_F4, SPLAT_BYTES, full);
+}
+
+// forward.cu:343-356 with the contraction of the reference SASS (SURVEY.md A.4): the Gaussian's exponent and alpha at
+// one pixel.  Shared by the forward and the contribution pass, so both take the same blend decisions bit for bit.
+__device__ __forceinline__ float pair_power(const float4 q0, const float4 q1, float pxf, float pyf) {
+  const float dx = q0.x - pxf, dy = q0.y - pyf;
+  const float t1 = __fmul_rn(__fmul_rn(dy, q1.x), dy);
+  const float t2 = __fmul_rn(dx, q0.z);
+  const float t3 = __fmul_rn(__fmul_rn(dx, q0.w), dy);
+  return __fmaf_rn(__fmaf_rn(dx, t2, t1), -0.5f, -t3);
+}
+__device__ __forceinline__ float pair_alpha(const float4 q1, float power) {
+  return fminf(0.99f, __fmul_rn(q1.y, expf(power)));
 }
 
 __device__ __forceinline__ void mbar_arrive(unsigned long long* bar) {
@@ -260,14 +274,9 @@ __global__ void __launch_bounds__(FWD_THREADS) k_render_fwd(int W, int H, int gx
         mask &= mask - 1;
         const float4* rec = sb + (base + bit) * SPLAT_F4;
         const float4 q0 = rec[0], q1 = rec[1];
-        // forward.cu:343-356 with the contraction of the reference SASS (SURVEY.md A.4)
-        const float dx = q0.x - pxf, dy = q0.y - pyf;
-        const float t1 = __fmul_rn(__fmul_rn(dy, q1.x), dy);
-        const float t2 = __fmul_rn(dx, q0.z);
-        const float t3 = __fmul_rn(__fmul_rn(dx, q0.w), dy);
-        const float power = __fmaf_rn(__fmaf_rn(dx, t2, t1), -0.5f, -t3);
+        const float power = pair_power(q0, q1, pxf, pyf);
         if (power > 0.0f) continue;
-        const float alpha = fminf(0.99f, __fmul_rn(q1.y, expf(power)));
+        const float alpha = pair_alpha(q1, power);
         if (alpha < 1.0f / 255.0f) continue;
         const float test_T = __fmul_rn(T, __fsub_rn(1.0f, alpha));
         if (test_T < 0.0001f) { T = -fabsf(T); continue; }
@@ -532,6 +541,123 @@ k_render_bwd(int W, int H, int gx, const float* __restrict__ bg, ImageView im, B
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// contribution statistics (gsr_contribution, DESIGN.md §7l): the forward's per-pixel walk replayed on its own buffers
+// ---------------------------------------------------------------------------------------------
+// A pixel whose walk ended on T (1 - alpha) < 1e-4 had T < CONTRIB_END_T when it ended: alpha <= 0.99 leaves
+// 1 - alpha >= 0.0099999, so the product of a T >= 0.0101 stays above 1e-4 after rounding.  A pixel whose final T is at
+// least this therefore never ended, and nothing behind its last contributor reached the transmittance test.
+constexpr float CONTRIB_END_T = 0.0101f;
+constexpr int CONTRIB_THREADS = TILE_PIX;  // one pixel per thread; warp w owns the forward's 8x4 block w
+// weight fixed point: a blend weight w <= 0.99 becomes round(w 2^32) < 2^32, a per-view sum of at most 2^26 pixels
+// stays below 2^58
+constexpr float CONTRIB_FIX = 4294967296.0f;
+
+__global__ void __launch_bounds__(CONTRIB_THREADS) k_render_contrib(int W, int H, int gx, ImageView im, BinView bin,
+                                                                    const float4* __restrict__ splat,
+                                                                    unsigned long long* __restrict__ fixed_w,
+                                                                    unsigned long long* __restrict__ count,
+                                                                    unsigned* __restrict__ max_w) {
+  __shared__ float4 recs[CONTRIB_THREADS * SPLAT_F4];
+  __shared__ unsigned cta_lim;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tile = (int)im.tile_order[blockIdx.x], tx = tile % gx, ty = tile / gx;
+  const uint2 range = im.tile_range[tile];
+  const int n = (int)(range.y - range.x);
+  if (n == 0) return;
+  const uint32_t* ids = bin.point_list + range.x;
+
+  const int sx0 = tx * TILE_X + (warp & 1) * 8, sy0 = ty * TILE_Y + (warp >> 1) * 4;
+  const int px = sx0 + (lane & 7), py = sy0 + (lane >> 3);
+  const bool inside = px < W && py < H;
+  const float pxf = (float)px, pyf = (float)py;
+  const float rx0 = (float)sx0, ry0 = (float)sy0;
+  const float rx1 = (float)min(sx0 + 7, W - 1), ry1 = (float)min(sy0 + 3, H - 1);
+  // list positions this pixel's walk can reach a transmittance test at: all of them if it may have ended, else up to
+  // its last contributor (n_contrib is 1 + that position)
+  int lim = 0;
+  if (inside) {
+    const size_t pid = (size_t)py * W + px;
+    lim = im.final_T[pid] < CONTRIB_END_T ? n : min(n, (int)im.n_contrib[pid]);
+  }
+  const int warp_lim = (int)__reduce_max_sync(FULL, (unsigned)lim);
+  if (tid == 0) cta_lim = 0;
+  __syncthreads();
+  if (lane == 0) atomicMax(&cta_lim, (unsigned)warp_lim);
+  __syncthreads();
+  const int nlim = (int)cta_lim;
+
+  // the forward's state of this pixel: a finished pixel has T < 0 (never again reaches the test)
+  float T = lim > 0 ? 1.0f : -1.0f;
+  for (int b0 = 0; b0 < nlim; b0 += CONTRIB_THREADS) {
+    const int cnt = min(CONTRIB_THREADS, nlim - b0);
+    if (tid < cnt) {
+      const float4* src = splat + (size_t)ids[b0 + tid] * SPLAT_F4;
+      recs[tid * SPLAT_F4 + 0] = src[0];
+      recs[tid * SPLAT_F4 + 1] = src[1];
+      recs[tid * SPLAT_F4 + 2] = src[2];
+    }
+    __syncthreads();
+    if (__any_sync(FULL, T > 0.f)) {
+      for (int base = 0; base < cnt && b0 + base < warp_lim; base += 32) {
+        const int j = base + lane;
+        bool keep = false;
+        if (j < cnt) {
+          const float4* cr = recs + j * SPLAT_F4;
+          keep = may_touch(cull_prep(cr[0], cr[1], cr[2].w), rx0, ry0, rx1, ry1);
+        }
+        unsigned mask = __ballot_sync(FULL, keep);
+        while (mask) {
+          const int bit = __ffs(mask) - 1;
+          mask &= mask - 1;
+          const float4* rec = recs + (base + bit) * SPLAT_F4;
+          const float4 q0 = rec[0], q1 = rec[1];
+          // the forward's decisions in its order: power > 0 and alpha < 1/255 skip the pair, then the pixel ends
+          // (counted, no weight) or blends with weight alpha T
+          bool reached = false;
+          float w = 0.f;
+          if (T > 0.f && b0 + base + bit < lim) {
+            const float power = pair_power(q0, q1, pxf, pyf);
+            if (!(power > 0.0f)) {
+              const float alpha = pair_alpha(q1, power);
+              if (!(alpha < 1.0f / 255.0f)) {
+                reached = true;
+                const float test_T = __fmul_rn(T, __fsub_rn(1.0f, alpha));
+                if (test_T < 0.0001f) {
+                  T = -T;
+                } else {
+                  w = __fmul_rn(alpha, T);
+                  T = test_T;
+                }
+              }
+            }
+          }
+          const unsigned rmask = __ballot_sync(FULL, reached);
+          if (rmask == 0) continue;
+          // exact integer sums over the block's 32 pixels (w < 2^32 in fixed point: 16-bit halves cannot overflow)
+          const unsigned q = __float2uint_rn(w * CONTRIB_FIX);
+          const unsigned hi = __reduce_add_sync(FULL, q >> 16), lo = __reduce_add_sync(FULL, q & 0xffffu);
+          const unsigned mx = __reduce_max_sync(FULL, __float_as_uint(w));  // w >= 0: bits order like values
+          if (lane == 0) {
+            const int g = __float_as_int(rec[2].z);
+            atomicAdd(&count[g], (unsigned long long)__popc(rmask));
+            const unsigned long long s = ((unsigned long long)hi << 16) + lo;
+            if (s) atomicAdd(&fixed_w[g], s);
+            if (mx) atomicMax(&max_w[g], mx);
+          }
+        }
+      }
+    }
+    if (__syncthreads_and(T < 0.f || b0 + CONTRIB_THREADS >= lim)) break;
+  }
+}
+
+// weight[i] += fixed_w[i] 2^-32 in double, views folded in stream order
+__global__ void k_contrib_fold(int P, const unsigned long long* __restrict__ fixed_w, double* __restrict__ weight) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < P && fixed_w[i]) weight[i] += (double)fixed_w[i] * (1.0 / 4294967296.0);
+}
+
 }  // namespace
 
 // Experiment knob (GSR_RENDER_PAD=<bytes>, read once): extra dynamic shared memory per compositing CTA.  It lowers the
@@ -577,3 +703,34 @@ void launch_render_bwd(int W, int H, int gx, int gy, const float* bg, ImageView 
 }
 
 }  // namespace gsr
+
+using namespace gsr;
+
+extern "C" {
+
+int gsr_contribution(int P, int64_t R, int width, int height, char* geom_buffer, const char* binning_buffer,
+                     const char* image_buffer, double* weight, int64_t* count, float* max_weight, void* stream) {
+  const char* fn = "gsr_contribution";
+  if (P < 0 || width <= 0 || height <= 0) return fail(fn, "P >= 0, width and height must be positive");
+  const int gx = (width + TILE_X - 1) / TILE_X, gy = (height + TILE_Y - 1) / TILE_Y;
+  if (gx > 65535 || gy > 65535) return fail(fn, "image too large");
+  if (P == 0) return 0;
+  if (!geom_buffer || !image_buffer || (R > 0 && !binning_buffer)) return fail(fn, "missing state buffers");
+  if (!weight || !count || !max_weight) return fail(fn, "weight, count and max_weight are required");
+  cudaStream_t st = (cudaStream_t)stream;
+  GeomView g = carve_geom(aligned_base(geom_buffer), P);
+  // the per-view fixed-point sums live in the backward's scratch (48 B per Gaussian), which a backward re-initialises
+  unsigned long long* fixed_w = reinterpret_cast<unsigned long long*>(g.grad);
+  if (!check(cudaMemsetAsync(fixed_w, 0, sizeof(unsigned long long) * (size_t)P, st), fn)) return -1;
+  if (R > 0) {
+    ImageView im = carve_image(aligned_base(const_cast<char*>(image_buffer)), width, height);
+    BinView b = carve_binning(aligned_base(const_cast<char*>(binning_buffer)), R);
+    k_render_contrib<<<gx * gy, CONTRIB_THREADS, 0, st>>>(width, height, gx, im, b, g.splat, fixed_w,
+                                                          reinterpret_cast<unsigned long long*>(count),
+                                                          reinterpret_cast<unsigned*>(max_weight));
+  }
+  k_contrib_fold<<<blocks(P, 256), 256, 0, st>>>(P, fixed_w, weight);
+  return launched(fn);
+}
+
+}  // extern "C"

@@ -85,6 +85,20 @@ int gsr_backward(int P, int D, int M, int64_t R, const float* background, int wi
                  float* dL_dcolor, float* dL_ddepth, float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh,
                  float* dL_dscale, float* dL_drot, int debug, void* stream);
 
+/* Contribution statistics of one rendered view (DESIGN.md §7l): the forward's per-pixel walk replayed on the buffers
+ * of a gsr_forward, gsr_forward_fused or gsr_forward_mip (exact or pipelined mode; R is the forward's return value,
+ * as for gsr_backward), with the forward's own blend and termination decisions.  For every Gaussian i it ADDS
+ *   weight[i]     += sum of w = alpha T over the pixels where i blended (per view in 32.32 fixed point, exact integer
+ *                    sums, then folded into the double in stream order);
+ *   count[i]      += the pixels whose walk reached the transmittance test at i: the pixels it blended plus the one
+ *                    pair per pixel that ended the pixel (T (1 - alpha) < 1e-4, no weight);
+ *   max_weight[i]  = max(max_weight[i], largest w), max_weight >= 0 on entry.
+ * Results do not depend on scheduling, tile order or speculation.  geom_buffer's backward scratch is used (a later
+ * gsr_backward of the same forward re-initialises it).  Shapes: weight double[P], count int64[P], max_weight
+ * float[P]. */
+int gsr_contribution(int P, int64_t R, int width, int height, char* geom_buffer, const char* binning_buffer,
+                     const char* image_buffer, double* weight, int64_t* count, float* max_weight, void* stream);
+
 /* Fused-activation variants -- the step immediately before the path in every caller (SURVEY.md §8f rank 1):
  * gaustudio's VanillaRenderer.get_gaussians_properties (gaustudio/renderers/vanilla_renderer.py:28-52) runs
  * exp(_scale), sigmoid(_opacity), normalize(_rot) and cat(_f_dc, _f_rest) as separate elementwise kernels on
