@@ -205,3 +205,16 @@ def scratch(dev):
         yield _scratch.slots
     finally:
         _scratch.slots = None
+
+
+def call_mesh(name, dev, *args):
+    """Entry point `name` that returns a mesh: `args` are its arguments before the trailing (scratch_alloc, scratch_user,
+    vertex_alloc, vertex_user, face_alloc, face_user, n_faces).  -> (vertices [V,3] float32, faces [F,3] int64) on
+    `dev`, both [0,3] when there is no mesh."""
+    nf = C.c_int64(0)
+    with scratch(dev) as bufs:
+        nv = call(name, dev, *args, ALLOC, 1, ALLOC, 2, ALLOC, 3, C.byref(nf))
+    F = nf.value
+    v = bufs[2].view(torch.float32).reshape(nv, 3) if nv else torch.empty(0, 3, device=dev)
+    f = bufs[3].view(torch.int64).reshape(F, 3) if F else torch.empty(0, 3, dtype=torch.int64, device=dev)
+    return v, f

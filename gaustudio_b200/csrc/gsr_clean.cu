@@ -31,8 +31,6 @@ constexpr int KMAX = 64;
 constexpr int BITS = 21;          // lattice cells per axis: 2^21; Morton keys of 63 bits
 constexpr int TOP = BITS - 1;     // coarsest level: 2 cells per axis
 constexpr int RMAX = 2;           // shells scanned at a level before moving up
-constexpr int RED_CTAS = 256;     // fixed grid of the reductions: their summation order never changes
-constexpr int RED_THREADS = 256;
 constexpr int KNN_THREADS = 256;  // 8 queries per block
 constexpr double MARGIN = 1e-9;   // lattice units: covers the rounding of (x - lo) * inv at |u| < 2^21
 constexpr double SLACK = 1.0 + 1e-12;  // relative: covers the rounding of a box distance against a point's
@@ -43,19 +41,6 @@ struct Lattice {
   int level;    // start level of the search
   int pad;
 };
-
-__device__ __forceinline__ double block_sum(double v, double* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  v = 0.0;
-  if (threadIdx.x == 0)
-    for (int k = 0; k < (int)(blockDim.x >> 5); k++) v += red[k];
-  __syncthreads();
-  return v;
-}
 
 // ---- lattice ----
 __global__ void __launch_bounds__(RED_THREADS) k_clean_box(int n, const float* __restrict__ xyz,
@@ -429,28 +414,29 @@ bool build_grid(const char* fn, int n, int k, const float* xyz, gsr_alloc_fn scr
   size_t sort_tmp = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
                                   (const int*)nullptr, (int*)nullptr, n, 0, 3 * BITS, st);
-  const size_t o_key = 0, o_key2 = align256((size_t)n * 8), o_idx = o_key2 + align256((size_t)n * 8),
-               o_idx2 = o_idx + align256((size_t)n * 4), o_sp = o_idx2 + align256((size_t)n * 4),
-               o_box = o_sp + align256((size_t)n * 16), o_lat = o_box + align256(RED_CTAS * 6 * 4),
-               o_hist = o_lat + 256, o_part = o_hist + 256, o_tmp = o_part + align256(RED_CTAS * 8),
-               total = o_tmp + align256(sort_tmp);
-  char* s = scratch_alloc(scratch_user, total);
-  if (!s) { fail(fn, "scratch allocation failed"); return false; }
-  unsigned long long* key = reinterpret_cast<unsigned long long*>(s + o_key);
-  unsigned long long* key2 = reinterpret_cast<unsigned long long*>(s + o_key2);
-  int* idx = reinterpret_cast<int*>(s + o_idx);
-  int* idx2 = reinterpret_cast<int*>(s + o_idx2);
-  float* box = reinterpret_cast<float*>(s + o_box);
-  int* hist = reinterpret_cast<int*>(s + o_hist);
-  g.sp = reinterpret_cast<float4*>(s + o_sp);
-  g.lat = reinterpret_cast<Lattice*>(s + o_lat);
+  unsigned long long *key, *key2;
+  int *idx, *idx2, *hist;
+  float* box;
+  char* tmp;
+  if (!carve_scratch(fn, scratch_alloc, scratch_user, [&](char*& p) {
+        take(p, key, n);
+        take(p, key2, n);
+        take(p, idx, n);
+        take(p, idx2, n);
+        take(p, g.sp, n);
+        take(p, box, RED_CTAS * 6);
+        take(p, g.lat, 1);
+        take(p, hist, BITS);
+        take(p, g.part, RED_CTAS);
+        take(p, tmp, sort_tmp);
+      }))
+    return false;
   g.key = key2;
-  g.part = reinterpret_cast<double*>(s + o_part);
   cudaMemsetAsync(hist, 0, BITS * sizeof(int), st);
   k_clean_box<<<RED_CTAS, RED_THREADS, 0, st>>>(n, xyz, box);
   k_clean_lattice<<<1, 1, 0, st>>>(box, g.lat);
   k_clean_keys<<<blocks(n, 256), 256, 0, st>>>(n, xyz, g.lat, key, idx);
-  cub::DeviceRadixSort::SortPairs(s + o_tmp, sort_tmp, (const unsigned long long*)key, key2, (const int*)idx, idx2, n,
+  cub::DeviceRadixSort::SortPairs(tmp, sort_tmp, (const unsigned long long*)key, key2, (const int*)idx, idx2, n,
                                   0, 3 * BITS, st);
   k_clean_gather<<<blocks(n, 256), 256, 0, st>>>(n, idx2, xyz, g.sp);
   const int t = max(1, min((k + 1) / 2, n));  // the points a start cell should hold: half of the k sought
@@ -460,11 +446,6 @@ bool build_grid(const char* fn, int n, int k, const float* xyz, gsr_alloc_fn scr
 }
 unsigned knn_blocks(int n) { return blocks(n, KNN_THREADS / 32); }
 
-bool n_ok(const char* fn, int64_t n) {
-  if (n >= 1 && n <= 0x7fffffffLL) return true;
-  fail(fn, "n must be in 1..2^31-1");
-  return false;
-}
 bool k_ok(const char* fn, int k) {
   if (k >= 1 && k <= KMAX) return true;
   fail(fn, "k must be in 1..64");
@@ -481,7 +462,7 @@ extern "C" {
 int gsr_clean_knn(int64_t n, const float* xyz, int k, gsr_alloc_fn scratch_alloc, void* scratch_user, int* index,
                   double* sq_dist, void* stream) {
   const char* fn = "gsr_clean_knn";
-  if (!n_ok(fn, n) || !k_ok(fn, k)) return -1;
+  if (!count_ok(fn, n, "n") || !k_ok(fn, k)) return -1;
   if (!xyz || !scratch_alloc || !index || !sq_dist) return fail(fn, "xyz, scratch_alloc, index and sq_dist are required");
   cudaStream_t st = (cudaStream_t)stream;
   Grid g;
@@ -494,7 +475,7 @@ int gsr_clean_knn(int64_t n, const float* xyz, int k, gsr_alloc_fn scratch_alloc
 int gsr_clean_statistical(int64_t n, const float* xyz, int k, double std_ratio, gsr_alloc_fn scratch_alloc,
                           void* scratch_user, double* avg_dist, double* stats, unsigned char* keep, void* stream) {
   const char* fn = "gsr_clean_statistical";
-  if (!n_ok(fn, n) || !k_ok(fn, k)) return -1;
+  if (!count_ok(fn, n, "n") || !k_ok(fn, k)) return -1;
   if (!(std_ratio > 0.0 && std_ratio < INFINITY)) return fail(fn, "std_ratio must be positive and finite");
   if (!xyz || !scratch_alloc || !avg_dist || !stats || !keep)
     return fail(fn, "xyz, scratch_alloc, avg_dist, stats and keep are required");
@@ -517,7 +498,7 @@ int gsr_clean_normal(int64_t n, const float* xyz, const float* normals, int k, d
                      gsr_alloc_fn scratch_alloc, void* scratch_user, double* mean_angle, unsigned char* keep,
                      void* stream) {
   const char* fn = "gsr_clean_normal";
-  if (!n_ok(fn, n) || !k_ok(fn, k)) return -1;
+  if (!count_ok(fn, n, "n") || !k_ok(fn, k)) return -1;
   if (!(angle_threshold > -INFINITY && angle_threshold < INFINITY)) return fail(fn, "angle_threshold must be finite");
   if (!xyz || !normals || !scratch_alloc || !mean_angle || !keep)
     return fail(fn, "xyz, normals, scratch_alloc, mean_angle and keep are required");
@@ -532,7 +513,7 @@ int gsr_clean_normal(int64_t n, const float* xyz, const float* normals, int k, d
 
 int gsr_dist2(int64_t n, const float* xyz, gsr_alloc_fn scratch_alloc, void* scratch_user, float* dist2, void* stream) {
   const char* fn = "gsr_dist2";
-  if (!n_ok(fn, n)) return -1;
+  if (!count_ok(fn, n, "n")) return -1;
   if (!xyz || !scratch_alloc || !dist2) return fail(fn, "xyz, scratch_alloc and dist2 are required");
   cudaStream_t st = (cudaStream_t)stream;
   Grid g;

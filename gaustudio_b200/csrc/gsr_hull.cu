@@ -4,16 +4,15 @@
 //   k_hull_carve                 one thread per grid node: the node leaves at the first camera whose insideView test
 //                                it fails (the reference's AND over every camera); camera records staged in shared
 //                                memory in chunks, every mask read from one uint8 buffer at the camera's offset
-//   k_hull_count / k_hull_emit   marching cubes of the occupancy (gsr_mc_tables.cuh), with the vertex of each
-//                                crossing edge at `threshold` from its empty end and mapped to the world in double
+//   k_mc_dense_count / _emit     marching cubes of the occupancy (gsr_mc.cuh), with the vertex of each crossing
+//                                edge at `threshold` from its empty end and mapped to the world in double
 //
 // Grid node g = (i res + j) res + k is the reference's meshgrid point (lin[j], lin[i], lin[k]) - translate: i walks
 // y, j walks x, k walks z, so the occupancy is the reference's `volume` array.  No atomics: the same inputs give the
 // same bits.
 #include "gsr_internal.cuh"
 #include "../../include/gsr.h"
-#include "gsr_mc_tables.cuh"
-#include <cub/cub.cuh>
+#include "gsr_mc.cuh"
 #include <cmath>
 
 namespace gsr {
@@ -21,7 +20,6 @@ namespace {
 
 constexpr int CARVE_THREADS = 256;
 constexpr int CAM_CHUNK = 128;  // camera records staged per round: 128 * (64 + 24) B = 11 KB
-constexpr int MAX_RES = 512;
 
 // np.linspace(start, stop, res)[i]: i * step + start (no contraction), the last node exactly stop
 __device__ __forceinline__ double lin(int i, int res, double start, double step, double stop) {
@@ -77,91 +75,37 @@ __global__ void __launch_bounds__(CARVE_THREADS) k_hull_carve(int res, double st
   if (g < N) occ[g] = filled ? 1 : 0;
 }
 
-// ---- marching cubes of the occupancy: node g is the base of cube g (all three indices < res - 1) ----
+// ---- marching cubes of the occupancy (gsr_mc.cuh) ----
 // Case bit k <=> corner k is empty, so the tables' triangles face the empty (carved) side in index space; the map to
 // the world swaps the first two axes (the reference's axis swap), a reflection, so each triangle is written reversed.
-__device__ __forceinline__ bool empty(unsigned char v) { return v == 0; }
-
-__global__ void __launch_bounds__(128) k_hull_count(int res, const unsigned char* __restrict__ occ,
-                                                    unsigned char* __restrict__ cube, unsigned char* __restrict__ edges,
-                                                    int* __restrict__ fcount, int* __restrict__ vcount) {
-  const long long N = (long long)res * res * res;
-  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g > N) return;
-  if (g == N) { fcount[N] = 0; vcount[N] = 0; return; }
-  const int c[3] = {(int)(g / ((long long)res * res)), (int)((g / res) % res), (int)(g % res)};
-  const long long step[3] = {(long long)res * res, res, 1};
-  const bool e0 = empty(occ[g]);
-  unsigned mask = 0;
-  for (int a = 0; a < 3; a++)
-    if (c[a] + 1 < res && empty(occ[g + step[a]]) != e0) mask |= 1u << a;
-  unsigned cs = 0;
-  const bool full = c[0] + 1 < res && c[1] + 1 < res && c[2] + 1 < res;
-  if (full)
-    for (int k = 0; k < 8; k++)
-      cs |= (unsigned)empty(occ[g + (k & 1) * step[0] + ((k >> 1) & 1) * step[1] + ((k >> 2) & 1) * step[2]]) << k;
-  cube[g] = (unsigned char)cs;
-  edges[g] = (unsigned char)mask;
-  fcount[g] = full ? mc_ntri[cs] : 0;
-  vcount[g] = __popc(mask);
-}
+struct Empty {
+  const unsigned char* __restrict__ occ;
+  __device__ bool operator()(long long g) const { return occ[g] == 0; }
+};
 
 // index coordinate q -> world: ((q / (res - 1)) (2 r) - r) - t, in double
 __device__ __forceinline__ float to_world(double q, double den, double two_r, double r, double t) {
   return __double2float_rn(__dsub_rn(__dsub_rn(__dmul_rn(__ddiv_rn(q, den), two_r), r), t));
 }
-
-__global__ void __launch_bounds__(128) k_hull_emit(int res, const unsigned char* __restrict__ occ,
-                                                   const unsigned char* __restrict__ cube,
-                                                   const unsigned char* __restrict__ edges,
-                                                   const int* __restrict__ vbase, const int* __restrict__ fbase,
-                                                   double threshold, double radius, double tx, double ty, double tz,
-                                                   float* __restrict__ verts, long long* __restrict__ faces) {
-  const long long N = (long long)res * res * res;
-  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= N) return;
-  const unsigned mask = edges[g], cs = cube[g];
-  const int nt = mc_ntri[cs];
-  if (!mask && !nt) return;
-  const int c[3] = {(int)(g / ((long long)res * res)), (int)((g / res) % res), (int)(g % res)};
-  const long long step[3] = {(long long)res * res, res, 1};
-  if (mask) {
+struct HullVertex {
+  const unsigned char* __restrict__ occ;
+  double threshold, radius, tx, ty, tz;
+  __device__ void operator()(int res, long long g, const int c[3], const long long*, unsigned mask, float* v) const {
     // PyMCubes' interpolation (x2 - x1)(iso - f1)/(f2 - f1) + x1 with f in {0, 1}: iso from an empty start node,
     // 1 - iso from a filled one
-    const double frac = empty(occ[g]) ? threshold : __dsub_rn(1.0, threshold);
+    const double frac = occ[g] == 0 ? threshold : __dsub_rn(1.0, threshold);
     const double den = (double)(res - 1), two_r = __dmul_rn(2.0, radius);
-    int vid = vbase[g];
     for (int a = 0; a < 3; a++) {
       if (!((mask >> a) & 1)) continue;
       double q[3] = {(double)c[0], (double)c[1], (double)c[2]};
       q[a] = __dadd_rn(q[a], frac);
-      float* v = verts + 3 * (size_t)vid;
       v[0] = to_world(q[1], den, two_r, radius, tx);  // world x walks the grid's second axis
       v[1] = to_world(q[0], den, two_r, radius, ty);
       v[2] = to_world(q[2], den, two_r, radius, tz);
-      vid++;
+      v += 3;
     }
   }
-  long long fo = fbase[g];
-  for (int t = 0; t < nt; t++, fo++)
-    for (int j = 0; j < 3; j++) {
-      const int e = mc_tri[cs][3 * t + j], c0 = mc_edge[e][0], a = mc_edge[e][2];
-      const long long go = g + (c0 & 1) * step[0] + ((c0 >> 1) & 1) * step[1] + ((c0 >> 2) & 1) * step[2];
-      faces[3 * fo + 2 - j] = vbase[go] + __popc(edges[go] & ((1u << a) - 1));
-    }
-}
-
-__global__ void k_hull_counts(const int* __restrict__ vbase, const int* __restrict__ fbase, long long N,
-                              long long* __restrict__ out) {
-  out[0] = vbase[N];
-  out[1] = fbase[N];
-}
-
-bool res_ok(const char* fn, int res) {
-  if (res >= 2 && res <= MAX_RES) return true;
-  fail(fn, "res must be in 2..512");
-  return false;
-}
+};
 
 }  // namespace
 }  // namespace gsr
@@ -197,36 +141,8 @@ int64_t gsr_hull_marching_cubes(int res, const unsigned char* occ, double thresh
   if (!occ) return fail(fn, "occ is required");
   if (!scratch_alloc || !vertex_alloc || !face_alloc || !n_faces)
     return fail(fn, "allocators and n_faces are required");
-  cudaStream_t st = (cudaStream_t)stream;
-  const long long N = (long long)res * res * res;
-  size_t scan_tmp = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (int*)nullptr, (int)(N + 1), st);
-  const size_t o_cube = 0, o_edges = align256(N), o_fb = o_edges + align256(N), o_vb = o_fb + align256((N + 1) * 4),
-               o_rb = o_vb + align256((N + 1) * 4), o_tmp = o_rb + 256, total = o_tmp + align256(scan_tmp);
-  char* s = scratch_alloc(scratch_user, total);
-  if (!s) return fail(fn, "scratch allocation failed");
-  unsigned char* cube = reinterpret_cast<unsigned char*>(s + o_cube);
-  unsigned char* edges = reinterpret_cast<unsigned char*>(s + o_edges);
-  int* fbase = reinterpret_cast<int*>(s + o_fb);
-  int* vbase = reinterpret_cast<int*>(s + o_vb);
-  long long* rb_dev = reinterpret_cast<long long*>(s + o_rb);
-  k_hull_count<<<blocks(N + 1, 128), 128, 0, st>>>(res, occ, cube, edges, fbase, vbase);
-  cub::DeviceScan::ExclusiveSum(s + o_tmp, scan_tmp, fbase, (int)(N + 1), st);
-  cub::DeviceScan::ExclusiveSum(s + o_tmp, scan_tmp, vbase, (int)(N + 1), st);
-  k_hull_counts<<<1, 1, 0, st>>>(vbase, fbase, N, rb_dev);
-  long long rb[2];
-  cudaMemcpyAsync(rb, rb_dev, sizeof(rb), cudaMemcpyDeviceToHost, st);
-  if (launched(fn)) return -1;
-  if (cudaStreamSynchronize(st) != cudaSuccess) { launched(fn); return -1; }
-  const long long V = rb[0], F = rb[1];
-  *n_faces = F;
-  if (V == 0 && F == 0) return 0;
-  char* verts = vertex_alloc(vertex_user, (size_t)V * 12);
-  char* faces = face_alloc(face_user, (size_t)F * 24);
-  if (!verts || !faces) return fail(fn, "output allocation failed");
-  k_hull_emit<<<blocks(N, 128), 128, 0, st>>>(res, occ, cube, edges, vbase, fbase, threshold, radius, tx, ty, tz,
-                                              reinterpret_cast<float*>(verts), reinterpret_cast<long long*>(faces));
-  return launched(fn) ? -1 : V;
+  return mc_dense<true>(fn, res, Empty{occ}, HullVertex{occ, threshold, radius, tx, ty, tz}, scratch_alloc,
+                       scratch_user, vertex_alloc, vertex_user, face_alloc, face_user, n_faces, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -438,18 +438,6 @@ __global__ void k_vox_colors(int ncell, const unsigned* __restrict__ cells, cons
   }
 }
 
-bool count_ok(const char* fn, int64_t n, const char* what) {
-  if (n >= 1 && n <= 0x7fffffffLL) return true;
-  fail(fn, std::string(what) + " must be in 1..2^31-1");
-  return false;
-}
-bool read_back(const char* fn, const long long* src, long long* dst, cudaStream_t st) {
-  cudaMemcpyAsync(dst, src, sizeof(long long), cudaMemcpyDeviceToHost, st);
-  if (launched(fn)) return false;
-  if (cudaStreamSynchronize(st) != cudaSuccess) { launched(fn); return false; }
-  return true;
-}
-
 }  // namespace
 }  // namespace gsr
 
@@ -479,14 +467,19 @@ int gsr_mesh_vertex_normals(int64_t nv, const float* verts, int64_t nf, const in
   size_t sort_tmp = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const int*)nullptr, (int*)nullptr, (const int*)nullptr,
                                   (int*)nullptr, m, 0, bits, st);
-  const size_t sz = align256((size_t)m * 4), total = 4 * sz + align256(sort_tmp);
-  char* s = scratch_alloc(scratch_user, total);
-  if (!s) return fail(fn, "scratch allocation failed");
-  int *key = reinterpret_cast<int*>(s), *face = reinterpret_cast<int*>(s + sz), *key2 = reinterpret_cast<int*>(s + 2 * sz),
-      *face2 = reinterpret_cast<int*>(s + 3 * sz);
+  int *key, *face, *key2, *face2;
+  char* tmp;
+  if (!carve_scratch(fn, scratch_alloc, scratch_user, [&](char*& p) {
+        take(p, key, m);
+        take(p, face, m);
+        take(p, key2, m);
+        take(p, face2, m);
+        take(p, tmp, sort_tmp);
+      }))
+    return -1;
   const long long* f64 = reinterpret_cast<const long long*>(faces);
   k_init_vn_pairs<<<blocks(m, 256), 256, 0, st>>>((int)nf, f64, key, face);
-  cub::DeviceRadixSort::SortPairs(s + 4 * sz, sort_tmp, (const int*)key, key2, (const int*)face, face2, m, 0, bits, st);
+  cub::DeviceRadixSort::SortPairs(tmp, sort_tmp, (const int*)key, key2, (const int*)face, face2, m, 0, bits, st);
   k_init_vn_sum<<<blocks(nv, 128), 128, 0, st>>>((int)nv, (int)nf, verts, f64, key2, face2, normals);
   return launched(fn);
 }
@@ -522,27 +515,33 @@ int64_t gsr_voxelize(int64_t nv, const double* verts, int64_t nf, const int64_t*
   // 1. columns per triangle
   size_t tmp = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, tmp, (long long*)nullptr, (long long*)nullptr, F + 1, st);
-  const size_t o_rb = align256((size_t)(F + 1) * 8), o_tmp = o_rb + 256;
-  char* s1 = alloc(column_user, o_tmp + align256(tmp));
-  if (!s1) return fail(fn, "scratch allocation failed");
-  long long* col_off = reinterpret_cast<long long*>(s1);
-  long long* rb = reinterpret_cast<long long*>(s1 + o_rb);
+  long long *col_off, *rb;
+  char* tmp1;
+  if (!carve_scratch(fn, alloc, column_user, [&](char*& p) {
+        take(p, col_off, F + 1);
+        take(p, rb, 1);
+        take(p, tmp1, tmp);
+      }))
+    return -1;
   k_vox_columns<<<blocks(F + 1, 256), 256, 0, st>>>(F, verts, f64, voxel_size, res, col_off);
-  cub::DeviceScan::ExclusiveSum(s1 + o_tmp, tmp, col_off, col_off, F + 1, st);
+  cub::DeviceScan::ExclusiveSum(tmp1, tmp, col_off, col_off, F + 1, st);
   k_vox_total<<<1, 1, 0, st>>>(col_off, F, rb);
-  if (!read_back(fn, rb, &C, st)) return -1;
+  if (read_back(fn, rb, &C, 1, st)) return -1;
   // 2. overlapping cells per column
   tmp = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, tmp, (long long*)nullptr, (long long*)nullptr, C + 1, st);
-  const size_t o_tmp2 = align256((size_t)(C + 1) * 8);
-  char* s2 = alloc(hit_user, o_tmp2 + align256(tmp));
-  if (!s2) return fail(fn, "scratch allocation failed");
-  long long* hits = reinterpret_cast<long long*>(s2);
+  long long* hits;
+  char* tmp2;
+  if (!carve_scratch(fn, alloc, hit_user, [&](char*& p) {
+        take(p, hits, C + 1);
+        take(p, tmp2, tmp);
+      }))
+    return -1;
   k_vox_hits<false><<<blocks(C + 1, 128), 128, 0, st>>>(F, C, verts, f64, voxel_size, res, col_off, hits, nullptr,
                                                          nullptr);
-  cub::DeviceScan::ExclusiveSum(s2 + o_tmp2, tmp, hits, hits, C + 1, st);
+  cub::DeviceScan::ExclusiveSum(tmp2, tmp, hits, hits, C + 1, st);
   k_vox_total<<<1, 1, 0, st>>>(hits, C, rb);
-  if (!read_back(fn, rb, &H, st)) return -1;
+  if (read_back(fn, rb, &H, 1, st)) return -1;
   *n_pairs = H;
   if (H == 0) return 0;
   if (H > 0x7fffffffLL) return fail(fn, "more than 2^31-1 (cell, triangle) pairs");
@@ -555,23 +554,29 @@ int64_t gsr_voxelize(int64_t nv, const double* verts, int64_t nf, const int64_t*
   cub::DeviceRunLengthEncode::Encode(nullptr, rle_tmp, (const unsigned*)nullptr, (unsigned*)nullptr, (int*)nullptr,
                                      (long long*)nullptr, (int)H, st);
   cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (int*)nullptr, (int*)nullptr, (int)H + 1, st);
-  const size_t a4 = align256((size_t)(H + 1) * 4), o_t = 6 * a4 + 256,
-               t_max = align256(std::max(sort_tmp, std::max(rle_tmp, scan_tmp)));
-  char* s3 = alloc(sort_user, o_t + t_max);
-  if (!s3) return fail(fn, "scratch allocation failed");
-  unsigned *cell = reinterpret_cast<unsigned*>(s3), *cell2 = reinterpret_cast<unsigned*>(s3 + a4),
-           *ucell = reinterpret_cast<unsigned*>(s3 + 2 * a4);
-  int *tri = reinterpret_cast<int*>(s3 + 3 * a4), *tri2 = reinterpret_cast<int*>(s3 + 4 * a4),
-      *cnt = reinterpret_cast<int*>(s3 + 5 * a4);
-  long long* nrun = reinterpret_cast<long long*>(s3 + 6 * a4);
+  unsigned *cell, *cell2, *ucell;
+  int *tri, *tri2, *cnt;
+  long long* nrun;
+  char* tmp3;
+  if (!carve_scratch(fn, alloc, sort_user, [&](char*& p) {
+        take(p, cell, H + 1);
+        take(p, cell2, H + 1);
+        take(p, ucell, H + 1);
+        take(p, tri, H + 1);
+        take(p, tri2, H + 1);
+        take(p, cnt, H + 1);
+        take(p, nrun, 1);
+        take(p, tmp3, std::max(sort_tmp, std::max(rle_tmp, scan_tmp)));
+      }))
+    return -1;
   k_vox_hits<true><<<blocks(C + 1, 128), 128, 0, st>>>(F, C, verts, f64, voxel_size, res, col_off, hits, cell, tri);
-  cub::DeviceRadixSort::SortPairs(s3 + o_t, sort_tmp, (const unsigned*)cell, cell2, (const int*)tri, tri2, (int)H, 0,
+  cub::DeviceRadixSort::SortPairs(tmp3, sort_tmp, (const unsigned*)cell, cell2, (const int*)tri, tri2, (int)H, 0,
                                   bits, st);
-  cudaMemsetAsync(cnt, 0, a4, st);
-  cub::DeviceRunLengthEncode::Encode(s3 + o_t, rle_tmp, (const unsigned*)cell2, ucell, cnt, nrun, (int)H, st);
-  if (!read_back(fn, nrun, &U, st)) return -1;
+  cudaMemsetAsync(cnt, 0, (size_t)(H + 1) * 4, st);
+  cub::DeviceRunLengthEncode::Encode(tmp3, rle_tmp, (const unsigned*)cell2, ucell, cnt, nrun, (int)H, st);
+  if (read_back(fn, nrun, &U, 1, st)) return -1;
   // counts -> offsets[U + 1] (cnt[U] is 0)
-  cub::DeviceScan::ExclusiveSum(s3 + o_t, scan_tmp, cnt, cnt, (int)U + 1, st);
+  cub::DeviceScan::ExclusiveSum(tmp3, scan_tmp, cnt, cnt, (int)U + 1, st);
   // 4. out: cells uint32[U] | offsets int32[U + 1] | triangles int32[H]
   char* out = alloc(out_user, (size_t)(2 * U + 1 + H) * 4);
   if (!out) return fail(fn, "output allocation failed");

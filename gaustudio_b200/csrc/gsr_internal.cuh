@@ -206,6 +206,36 @@ __device__ __forceinline__ int cta_exclusive_scan(int v, int* total) {
 }
 }  // namespace cta
 
+// CTA-wide sum / max of one double per thread, in a fixed order (warp shuffles, then thread 0 over the warps); the
+// result is valid in thread 0.  The per-point reductions of gsr_sap.cu and gsr_clean.cu run RED_CTAS CTAs of
+// RED_THREADS threads and add the RED_CTAS partials in one CTA: a fixed grid, so their summation order never changes.
+constexpr int RED_CTAS = 256;
+constexpr int RED_THREADS = 256;
+__device__ __forceinline__ double block_sum(double v, double* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  v = 0.0;
+  if (threadIdx.x == 0)
+    for (int k = 0; k < (int)(blockDim.x >> 5); k++) v += red[k];
+  __syncthreads();
+  return v;
+}
+__device__ __forceinline__ double block_max(double v, double* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_down_sync(0xffffffffu, v, o));
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  v = 0.0;
+  if (threadIdx.x == 0)
+    for (int k = 0; k < (int)(blockDim.x >> 5); k++) v = fmax(v, red[k]);
+  __syncthreads();
+  return v;
+}
+
 __device__ __forceinline__ int subbin_of(int gaussian_idx) { return gaussian_idx & (SUBBINS - 1); }
 __device__ __forceinline__ uint2 pack_rect(int xmin, int ymin, int xmax, int ymax) {
   return make_uint2((unsigned)xmin | ((unsigned)xmax << 16), (unsigned)ymin | ((unsigned)ymax << 16));
@@ -336,6 +366,25 @@ inline int launched(const char* entry) {
 }
 inline unsigned blocks(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 bool kernel_size_ok(float k);  // width of a Mip filter: finite and >= 0
+// a count the kernels index with int: "<what> must be in 1..2^31-1" otherwise
+inline bool count_ok(const char* fn, int64_t n, const char* what) {
+  if (n >= 1 && n <= 0x7fffffffLL) return true;
+  fail(fn, std::string(what) + " must be in 1..2^31-1");
+  return false;
+}
+// the edge of a dense grid (visual hull, Shape-as-Points)
+inline bool res_ok(const char* fn, int res) {
+  if (res >= 2 && res <= 512) return true;
+  fail(fn, "res must be in 2..512");
+  return false;
+}
+// copies n device words to the host on st and synchronises: 0, or -1 with the entry's error set
+template <typename T> inline int read_back(const char* fn, const T* src, T* dst, size_t n, cudaStream_t st) {
+  cudaMemcpyAsync(dst, src, n * sizeof(T), cudaMemcpyDeviceToHost, st);
+  if (launched(fn)) return -1;
+  if (cudaStreamSynchronize(st) != cudaSuccess) { launched(fn); return -1; }
+  return 0;
+}
 
 inline size_t align256(size_t v) { return (v + 255) / 256 * 256; }
 // carves `count` elements from p at its next 256-byte boundary and advances p past them
@@ -345,6 +394,18 @@ template <typename T> inline void take(char*& p, T*& out, size_t count) {
   p += count * sizeof(T);
 }
 inline char* aligned_base(char* p) { return reinterpret_cast<char*>(align256(reinterpret_cast<size_t>(p))); }
+// Asks `alloc` for one scratch block and carves it: `layout(p)` takes every array from p with take().  The layout runs
+// from a null base to size the block (255 bytes more cover an allocation that is not 256-byte aligned), then on the
+// allocation.  false: the allocation failed, with the entry's error set.
+template <typename Layout>
+inline bool carve_scratch(const char* fn, char* (*alloc)(void*, size_t), void* user, Layout layout) {
+  char* p = nullptr;
+  layout(p);
+  char* base = alloc(user, reinterpret_cast<size_t>(p) + 255);
+  if (!base) { fail(fn, "scratch allocation failed"); return false; }
+  layout(base);
+  return true;
+}
 // the projection kernels move a Gaussian's quaternion (and its gradient, and dL_dconic) as one float4
 inline bool misaligned16(const void* p) { return (reinterpret_cast<size_t>(p) & 15) != 0; }
 

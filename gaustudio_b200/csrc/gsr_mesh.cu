@@ -6,7 +6,8 @@
 //   k_tsdf_rays<true>    add the samples: fixed-point int64 sums + int32 counts, 64-bit atomics
 //   k_mc_cubes           per voxel: marching-cubes case of the cube whose corners are v + {0,1}^3, face count
 //   k_mc_edges           per voxel: crossing edges it owns (+x, +y, +z) that an active cube uses, vertex count
-//   k_mc_emit            vertices (shared, one per crossing edge) and faces, at their scanned offsets
+//   k_mc_emit            vertices (shared, one per crossing edge) and faces, at their scanned offsets; the scans,
+//                        the one read-back, the outputs and the face lookup are those of gsr_mc.cuh
 //   k_edge_keys / k_union / k_label   triangle components joined by shared edges (union-find)
 //
 // Claiming and adding are separate launches over the same DDA, so no thread ever waits on a table slot another
@@ -15,8 +16,7 @@
 // numpy restatement (oracle/tsdf_oracle.py) bit for bit.
 #include "gsr_internal.cuh"
 #include "../../include/gsr.h"
-#include "gsr_mc_tables.cuh"
-#include <cub/cub.cuh>
+#include "gsr_mc.cuh"
 #include <cmath>
 #include <string>
 
@@ -342,14 +342,9 @@ __global__ void __launch_bounds__(128) k_mc_emit(MeshCtx m, long long N, const i
       for (int j = 0; j < 3; j++) {
         const int e = mc_tri[c][3 * t + j], c0 = mc_edge[e][0], a = mc_edge[e][2];
         const long long go = voxel_g(m, x + (c0 & 1), y + ((c0 >> 1) & 1), z + ((c0 >> 2) & 1));
-        faces[3 * fo + j] = m.vbase[go] + __popc(m.edges[go] & ((1u << a) - 1));
+        faces[3 * fo + j] = mc_vertex(m.vbase, m.edges, go, a);
       }
   }
-}
-
-__global__ void k_readback(TsdfView v, const int* vbase, const int* fbase, long long N, unsigned long long* out) {
-  out[0] = v.hdr->n_bricks; out[1] = v.hdr->dropped; out[2] = v.hdr->far;
-  out[3] = vbase ? (unsigned long long)vbase[N] : 0; out[4] = fbase ? (unsigned long long)fbase[N] : 0;
 }
 
 __global__ void k_export(TsdfView v, const unsigned long long* __restrict__ sorted_keys,
@@ -408,32 +403,35 @@ bool cap_ok(const char* fn, long long cap) {
   return false;
 }
 
-// Sorts the bricks by key into scratch; returns the carved scratch pointers or false (error set)
+// Sorts the bricks by key into scratch; `rest(p)` takes the caller's arrays from the same block, after the sort's own
 struct SortedBricks {
   unsigned long long* keys;
   int* idx;
-  char* rest;  // scratch after the sort's own arrays
 };
-bool sort_bricks(const char* fn, const TsdfView& v, gsr_alloc_fn alloc, void* user, size_t extra, SortedBricks& out,
+template <typename Rest>
+bool sort_bricks(const char* fn, const TsdfView& v, gsr_alloc_fn alloc, void* user, Rest rest, SortedBricks& out,
                  cudaStream_t st) {
   const int cap = (int)v.cap;
   size_t sort_tmp = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const unsigned long long*)nullptr,
                                   (unsigned long long*)nullptr, (const int*)nullptr, (int*)nullptr, cap, 0, 64, st);
-  const size_t o_keys = 0, o_iota = align256((size_t)cap * 8), o_idx = o_iota + align256((size_t)cap * 4),
-               o_tmp = o_idx + align256((size_t)cap * 4), o_rest = o_tmp + align256(sort_tmp);
-  char* s = alloc(user, o_rest + extra);
-  if (!s) { fail(fn, "scratch allocation failed"); return false; }
-  out.keys = reinterpret_cast<unsigned long long*>(s + o_keys);
-  out.idx = reinterpret_cast<int*>(s + o_idx);
-  out.rest = s + o_rest;
-  int* iota = reinterpret_cast<int*>(s + o_iota);
+  int* iota;
+  char* tmp;
+  if (!carve_scratch(fn, alloc, user, [&](char*& p) {
+        take(p, out.keys, cap);
+        take(p, iota, cap);
+        take(p, out.idx, cap);
+        take(p, tmp, sort_tmp);
+        rest(p);
+      }))
+    return false;
   k_iota<<<blocks(cap, 256), 256, 0, st>>>(cap, iota);
-  cub::DeviceRadixSort::SortPairs(s + o_tmp, sort_tmp, (const unsigned long long*)v.brick_keys, out.keys,
-                                  (const int*)iota, out.idx, cap, 0, 64, st);
+  cub::DeviceRadixSort::SortPairs(tmp, sort_tmp, (const unsigned long long*)v.brick_keys, out.keys, (const int*)iota,
+                                  out.idx, cap, 0, 64, st);
   return launched(fn) == 0;
 }
 
+// rb: the header's n_bricks, dropped, far
 bool volume_ok(const char* fn, const unsigned long long* rb, long long cap) {
   if (rb[0] > (unsigned long long)cap || rb[1]) {
     fail(fn, (rb[1] ? "the TSDF volume needs more than " : "the TSDF volume needs ") + std::to_string(rb[0]) +
@@ -507,43 +505,38 @@ int64_t gsr_tsdf_extract(void* state, int64_t capacity_bricks, double min_weight
   TsdfView v;
   tsdf_layout(static_cast<char*>(state), capacity_bricks, &v);
   const long long N = capacity_bricks * BRICK_VOX;
-  size_t scan_tmp = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (int*)nullptr, (int)(N + 1), st);
-  const size_t o_rank = 0, o_cube = align256((size_t)capacity_bricks * 4), o_edges = o_cube + align256(N * 2),
-               o_fb = o_edges + align256(N), o_vb = o_fb + align256((N + 1) * 4), o_rb = o_vb + align256((N + 1) * 4),
-               o_tmp = o_rb + 256, extra = o_tmp + align256(scan_tmp);
+  int* rank_of;
+  unsigned short* cube;
+  unsigned char* edges;
+  McScan sc;
   SortedBricks sb;
-  if (!sort_bricks(fn, v, scratch_alloc, scratch_user, extra, sb, st)) return -1;
-  char* s = sb.rest;
+  if (!sort_bricks(fn, v, scratch_alloc, scratch_user, [&](char*& p) {
+        take(p, rank_of, capacity_bricks);
+        take(p, cube, N);
+        take(p, edges, N);
+        take(p, sc, N, st);
+      }, sb, st))
+    return -1;
   MeshCtx m;
   m.v = v;
   m.sorted_keys = sb.keys;
-  int* rank_of = reinterpret_cast<int*>(s + o_rank);
-  unsigned short* cube = reinterpret_cast<unsigned short*>(s + o_cube);
-  unsigned char* edges = reinterpret_cast<unsigned char*>(s + o_edges);
-  int* fbase = reinterpret_cast<int*>(s + o_fb);
-  int* vbase = reinterpret_cast<int*>(s + o_vb);
-  unsigned long long* rb_dev = reinterpret_cast<unsigned long long*>(s + o_rb);
-  m.rank_of = rank_of; m.cube = cube; m.edges = edges; m.vbase = vbase; m.min_weight = min_weight;
+  m.rank_of = rank_of; m.cube = cube; m.edges = edges; m.vbase = sc.vbase; m.min_weight = min_weight;
   k_rank<<<blocks(capacity_bricks, 256), 256, 0, st>>>(v, sb.idx, rank_of);
-  k_mc_cubes<<<blocks(N + 1, 128), 128, 0, st>>>(m, N, cube, fbase);
-  k_mc_edges<<<blocks(N + 1, 128), 128, 0, st>>>(m, N, edges, vbase);
-  cub::DeviceScan::ExclusiveSum(s + o_tmp, scan_tmp, fbase, (int)(N + 1), st);
-  cub::DeviceScan::ExclusiveSum(s + o_tmp, scan_tmp, vbase, (int)(N + 1), st);
-  k_readback<<<1, 1, 0, st>>>(v, vbase, fbase, N, rb_dev);
+  k_mc_cubes<<<blocks(N + 1, 128), 128, 0, st>>>(m, N, cube, sc.fbase);
+  k_mc_edges<<<blocks(N + 1, 128), 128, 0, st>>>(m, N, edges, sc.vbase);
+  mc_scan(sc, N, st);
+  // the volume's counters ride along in the same read-back: its refusals come before any output is allocated
+  cudaMemcpyAsync(sc.rb + 2, &v.hdr->n_bricks, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st);
   unsigned long long rb[5];
-  cudaMemcpyAsync(rb, rb_dev, sizeof(rb), cudaMemcpyDeviceToHost, st);
-  if (launched(fn)) return -1;
-  if (cudaStreamSynchronize(st) != cudaSuccess) { launched(fn); return -1; }
-  if (!volume_ok(fn, rb, capacity_bricks)) return -1;
-  const long long V = (long long)rb[3], F = (long long)rb[4];
-  *n_faces = F;
-  if (V == 0 && F == 0) return 0;
-  char* verts = vertex_alloc(vertex_user, (size_t)V * 12);
-  char* faces = face_alloc(face_user, (size_t)F * 24);
-  if (!verts || !faces) return fail(fn, "output allocation failed");
-  k_mc_emit<<<blocks(N, 128), 128, 0, st>>>(m, N, fbase, reinterpret_cast<float*>(verts),
-                                            reinterpret_cast<long long*>(faces));
+  if (read_back(fn, sc.rb, rb, 5, st)) return -1;
+  if (!volume_ok(fn, rb + 2, capacity_bricks)) return -1;
+  const long long V = (long long)rb[0];
+  float* verts;
+  long long* faces;
+  const int out = mc_outputs(fn, V, (long long)rb[1], n_faces, vertex_alloc, vertex_user, face_alloc, face_user, verts,
+                             faces);
+  if (out <= 0) return out;
+  k_mc_emit<<<blocks(N, 128), 128, 0, st>>>(m, N, sc.fbase, verts, faces);
   return launched(fn) ? -1 : V;
 }
 
@@ -557,13 +550,9 @@ int64_t gsr_tsdf_export(void* state, int64_t capacity_bricks, gsr_alloc_fn scrat
   TsdfView v;
   tsdf_layout(static_cast<char*>(state), capacity_bricks, &v);
   SortedBricks sb;
-  if (!sort_bricks(fn, v, scratch_alloc, scratch_user, 256, sb, st)) return -1;
-  unsigned long long* rb_dev = reinterpret_cast<unsigned long long*>(sb.rest);
-  k_readback<<<1, 1, 0, st>>>(v, nullptr, nullptr, 0, rb_dev);
-  unsigned long long rb[5];
-  cudaMemcpyAsync(rb, rb_dev, sizeof(rb), cudaMemcpyDeviceToHost, st);
-  if (launched(fn)) return -1;
-  if (cudaStreamSynchronize(st) != cudaSuccess) { launched(fn); return -1; }
+  if (!sort_bricks(fn, v, scratch_alloc, scratch_user, [](char*&) {}, sb, st)) return -1;
+  unsigned long long rb[3];
+  if (read_back(fn, &v.hdr->n_bricks, rb, 3, st)) return -1;
   if (!volume_ok(fn, rb, capacity_bricks)) return -1;
   const long long n = (long long)rb[0];
   if (n > 0 && (brick_keys || sums || weights))
@@ -584,17 +573,20 @@ int gsr_mesh_face_components(int64_t n_faces, const int64_t* faces, int64_t n_ve
   size_t sort_tmp = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
                                   (const int*)nullptr, (int*)nullptr, (int)n, 0, 64, st);
-  const size_t o_k = 0, o_v = align256(n * 8), o_k2 = o_v + align256(n * 4), o_v2 = o_k2 + align256(n * 8),
-               o_p = o_v2 + align256(n * 4), o_t = o_p + align256(F * 4), total = o_t + align256(sort_tmp);
-  char* s = scratch_alloc(scratch_user, total);
-  if (!s) return fail(fn, "scratch allocation failed");
-  auto* keys = reinterpret_cast<unsigned long long*>(s + o_k);
-  auto* vals = reinterpret_cast<int*>(s + o_v);
-  auto* keys2 = reinterpret_cast<unsigned long long*>(s + o_k2);
-  auto* vals2 = reinterpret_cast<int*>(s + o_v2);
-  int* parent = reinterpret_cast<int*>(s + o_p);
+  unsigned long long *keys, *keys2;
+  int *vals, *vals2, *parent;
+  char* tmp;
+  if (!carve_scratch(fn, scratch_alloc, scratch_user, [&](char*& p) {
+        take(p, keys, n);
+        take(p, vals, n);
+        take(p, keys2, n);
+        take(p, vals2, n);
+        take(p, parent, F);
+        take(p, tmp, sort_tmp);
+      }))
+    return -1;
   k_edge_keys<<<blocks(n, 256), 256, 0, st>>>(F, reinterpret_cast<const long long*>(faces), n_vertices, keys, vals);
-  cub::DeviceRadixSort::SortPairs(s + o_t, sort_tmp, (const unsigned long long*)keys, keys2, (const int*)vals, vals2,
+  cub::DeviceRadixSort::SortPairs(tmp, sort_tmp, (const unsigned long long*)keys, keys2, (const int*)vals, vals2,
                                   (int)n, 0, 64, st);
   k_iota<<<blocks(F, 256), 256, 0, st>>>((int)F, parent);
   k_union<<<blocks(n, 256), 256, 0, st>>>(n, keys2, vals2, parent);

@@ -7,48 +7,18 @@
 //   k_sap_splat                                 per grid node: trilinear gather from its 8 neighbouring cells
 //   k_sap_spectral                              one pass over the half spectrum: Phi = -i sum_d w_d G N_d / (-|w|^2 + 1e-6)
 //   k_sap_interp / k_sap_offset / k_sap_psi     offset = mean of phi at the points; psi = tanh(-(phi - offset)/|fv0|/2)
-//   k_dmc_count / k_dmc_emit                    marching cubes of psi at 0 over the dense grid (gsr_mc_tables.cuh)
+//   k_mc_dense_count / _emit                    marching cubes of psi at 0 over the dense grid (gsr_mc.cuh)
 //
 // The forward and inverse FFTs between the splat and the spectral pass, and between the spectral pass and the shift,
 // are cuFFT through torch.fft (gaustudio_b200/extract.py).  Every sum is formed in a fixed order (no float atomics),
 // so the same inputs give the same bits.
 #include "gsr_internal.cuh"
 #include "../../include/gsr.h"
-#include "gsr_mc_tables.cuh"
-#include <cub/cub.cuh>
+#include "gsr_mc.cuh"
 #include <cmath>
 
 namespace gsr {
 namespace {
-
-constexpr int RED_CTAS = 256;     // fixed grid of the per-point reductions: their summation order never changes
-constexpr int RED_THREADS = 256;
-constexpr int MAX_RES = 512;
-
-__device__ __forceinline__ double block_sum(double v, double* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  v = 0.0;
-  if (threadIdx.x == 0)
-    for (int k = 0; k < (int)(blockDim.x >> 5); k++) v += red[k];
-  __syncthreads();
-  return v;
-}
-__device__ __forceinline__ double block_max(double v, double* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_down_sync(0xffffffffu, v, o));
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  v = 0.0;
-  if (threadIdx.x == 0)
-    for (int k = 0; k < (int)(blockDim.x >> 5); k++) v = fmax(v, red[k]);
-  __syncthreads();
-  return v;
-}
 
 // ---- normalisation: transform = (c.x, c.y, c.z, s) as float32, the reference's float32 centre and scale ----
 __global__ void __launch_bounds__(RED_THREADS) k_sap_sum(long long n, const float* __restrict__ xyz,
@@ -236,91 +206,34 @@ __global__ void k_sap_psi(long long N, const float* __restrict__ phi, const doub
   psi[g] = tanhf(__fmul_rn(__fdiv_rn(-__fsub_rn(phi[g], off), fv0), 0.5f));
 }
 
-// ---- marching cubes over the dense grid: node g = (x res + y) res + z is the base of cube g (x, y, z < res - 1) ----
+// ---- marching cubes over the dense grid (gsr_mc.cuh): node g = (x res + y) res + z ----
 // psi is positive outside the shape (on the side the input normals point; the grid corner has tanh(0.5)) and the
-// tables' convention (case bit k <=> psi >= 0 at corner k, triangles facing psi > 0) gives outward faces.  Every
-// crossing edge of the grid lies on a cube, so each one owns a vertex.
-__device__ __forceinline__ bool outside(float psi) { return psi >= 0.0f; }
-
-__global__ void __launch_bounds__(128) k_dmc_count(int res, const float* __restrict__ psi,
-                                                   unsigned char* __restrict__ cube, unsigned char* __restrict__ edges,
-                                                   int* __restrict__ fcount, int* __restrict__ vcount) {
-  const long long N = (long long)res * res * res;
-  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g > N) return;
-  if (g == N) { fcount[N] = 0; vcount[N] = 0; return; }
-  const int x = (int)(g / ((long long)res * res)), y = (int)((g / res) % res), z = (int)(g % res);
-  const long long step[3] = {(long long)res * res, res, 1};
-  const int c[3] = {x, y, z};
-  const bool out0 = outside(psi[g]);
-  unsigned mask = 0;
-  for (int a = 0; a < 3; a++)
-    if (c[a] + 1 < res && outside(psi[g + step[a]]) != out0) mask |= 1u << a;
-  unsigned cs = 0;
-  const bool full = x + 1 < res && y + 1 < res && z + 1 < res;
-  if (full)
-    for (int k = 0; k < 8; k++)
-      cs |= (unsigned)outside(psi[g + (k & 1) * step[0] + ((k >> 1) & 1) * step[1] + ((k >> 2) & 1) * step[2]]) << k;
-  cube[g] = (unsigned char)cs;
-  edges[g] = (unsigned char)mask;
-  fcount[g] = full ? mc_ntri[cs] : 0;
-  vcount[g] = __popc(mask);
-}
-
-__global__ void __launch_bounds__(128) k_dmc_emit(int res, const float* __restrict__ psi,
-                                                  const unsigned char* __restrict__ cube,
-                                                  const unsigned char* __restrict__ edges, const int* __restrict__ vbase,
-                                                  const int* __restrict__ fbase, const float* __restrict__ transform,
-                                                  float* __restrict__ verts, long long* __restrict__ faces) {
-  const long long N = (long long)res * res * res;
-  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= N) return;
-  const unsigned mask = edges[g], cs = cube[g];
-  const int nt = mc_ntri[cs];
-  if (!mask && !nt) return;
-  const int c[3] = {(int)(g / ((long long)res * res)), (int)((g / res) % res), (int)(g % res)};
-  const long long step[3] = {(long long)res * res, res, 1};
-  if (mask) {
+// tables' convention (case bit k <=> psi >= 0 at corner k, triangles facing psi > 0) gives outward faces.
+struct Outside {
+  const float* __restrict__ psi;
+  __device__ bool operator()(long long g) const { return psi[g] >= 0.0f; }
+};
+struct SapVertex {
+  const float* __restrict__ psi;
+  const float* __restrict__ transform;
+  __device__ void operator()(int res, long long g, const int c[3], const long long step[3], unsigned mask,
+                             float* v) const {
     const float s = transform[3];
     const double f0 = psi[g];
-    int vid = vbase[g];
     for (int a = 0; a < 3; a++) {
       if (!((mask >> a) & 1)) continue;
       const double f1 = psi[g + step[a]];
       const double t = __ddiv_rn(f0, __dsub_rn(f0, f1));
       for (int k = 0; k < 3; k++) {
         // index coordinate / res (mc_from_psr, real_scale=False), then ShapeAsPoints.transform(inverse=True)
-        const float v = __double2float_rn(__ddiv_rn(k == a ? __dadd_rn((double)c[k], t) : (double)c[k], (double)res));
-        verts[3 * (size_t)vid + k] = __fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(v, 2.0f), 1.0f), s), transform[k]);
+        const float u = __double2float_rn(__ddiv_rn(k == a ? __dadd_rn((double)c[k], t) : (double)c[k], (double)res));
+        v[k] = __fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(u, 2.0f), 1.0f), s), transform[k]);
       }
-      vid++;
+      v += 3;
     }
   }
-  long long fo = fbase[g];
-  for (int t = 0; t < nt; t++, fo++)
-    for (int j = 0; j < 3; j++) {
-      const int e = mc_tri[cs][3 * t + j], c0 = mc_edge[e][0], a = mc_edge[e][2];
-      const long long go = g + (c0 & 1) * step[0] + ((c0 >> 1) & 1) * step[1] + ((c0 >> 2) & 1) * step[2];
-      faces[3 * fo + j] = vbase[go] + __popc(edges[go] & ((1u << a) - 1));
-    }
-}
+};
 
-__global__ void k_dmc_counts(const int* __restrict__ vbase, const int* __restrict__ fbase, long long N,
-                             long long* __restrict__ out) {
-  out[0] = vbase[N];
-  out[1] = fbase[N];
-}
-
-bool n_ok(const char* fn, int64_t n) {
-  if (n >= 1 && n <= 0x7fffffffLL) return true;
-  fail(fn, "n must be in 1..2^31-1");
-  return false;
-}
-bool res_ok(const char* fn, int res) {
-  if (res >= 2 && res <= MAX_RES) return true;
-  fail(fn, "res must be in 2..512");
-  return false;
-}
 int end_bit(long long cells) {
   int b = 1;
   while ((1LL << b) < cells) b++;
@@ -337,7 +250,7 @@ extern "C" {
 int gsr_sap_normalize(int64_t n, const float* xyz, gsr_alloc_fn scratch_alloc, void* scratch_user, float* points01,
                       float* transform, void* stream) {
   const char* fn = "gsr_sap_normalize";
-  if (!n_ok(fn, n)) return -1;
+  if (!count_ok(fn, n, "n")) return -1;
   if (!xyz || !points01 || !transform || !scratch_alloc)
     return fail(fn, "xyz, points01, transform and scratch_alloc are required");
   cudaStream_t st = (cudaStream_t)stream;
@@ -354,7 +267,7 @@ int gsr_sap_normalize(int64_t n, const float* xyz, gsr_alloc_fn scratch_alloc, v
 int gsr_sap_splat(int64_t n, const float* points01, const float* normals, int res, gsr_alloc_fn scratch_alloc,
                   void* scratch_user, float* grid, void* stream) {
   const char* fn = "gsr_sap_splat";
-  if (!n_ok(fn, n) || !res_ok(fn, res)) return -1;
+  if (!count_ok(fn, n, "n") || !res_ok(fn, res)) return -1;
   if (!points01 || !normals || !grid || !scratch_alloc)
     return fail(fn, "points01, normals, grid and scratch_alloc are required");
   cudaStream_t st = (cudaStream_t)stream;
@@ -364,23 +277,25 @@ int gsr_sap_splat(int64_t n, const float* points01, const float* normals, int re
   cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const unsigned*)nullptr, (unsigned*)nullptr, (const int*)nullptr,
                                   (int*)nullptr, (int)n, 0, bits, st);
   cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (int*)nullptr, (int)(cells + 1), st);
-  const size_t o_start = 0, o_key = align256((cells + 1) * 4), o_key2 = o_key + align256(n * 4),
-               o_idx = o_key2 + align256(n * 4), o_idx2 = o_idx + align256(n * 4), o_sp = o_idx2 + align256(n * 4),
-               o_sn = o_sp + align256(n * 12), o_tmp = o_sn + align256(n * 12),
-               total = o_tmp + align256(sort_tmp > scan_tmp ? sort_tmp : scan_tmp);
-  char* s = scratch_alloc(scratch_user, total);
-  if (!s) return fail(fn, "scratch allocation failed");
-  int* start = reinterpret_cast<int*>(s + o_start);
-  unsigned* key = reinterpret_cast<unsigned*>(s + o_key);
-  unsigned* key2 = reinterpret_cast<unsigned*>(s + o_key2);
-  int* idx = reinterpret_cast<int*>(s + o_idx);
-  int* idx2 = reinterpret_cast<int*>(s + o_idx2);
-  float* sp = reinterpret_cast<float*>(s + o_sp);
-  float* sn = reinterpret_cast<float*>(s + o_sn);
+  int *start, *idx, *idx2;
+  unsigned *key, *key2;
+  float *sp, *sn;
+  char* tmp;
+  if (!carve_scratch(fn, scratch_alloc, scratch_user, [&](char*& p) {
+        take(p, start, cells + 1);
+        take(p, key, n);
+        take(p, key2, n);
+        take(p, idx, n);
+        take(p, idx2, n);
+        take(p, sp, 3 * n);
+        take(p, sn, 3 * n);
+        take(p, tmp, sort_tmp > scan_tmp ? sort_tmp : scan_tmp);
+      }))
+    return -1;
   cudaMemsetAsync(start, 0, (cells + 1) * 4, st);
   k_sap_cells<<<blocks(n, 256), 256, 0, st>>>(n, points01, res, key, idx, start);
-  cub::DeviceScan::ExclusiveSum(s + o_tmp, scan_tmp, start, (int)(cells + 1), st);
-  cub::DeviceRadixSort::SortPairs(s + o_tmp, sort_tmp, (const unsigned*)key, key2, (const int*)idx, idx2, (int)n, 0,
+  cub::DeviceScan::ExclusiveSum(tmp, scan_tmp, start, (int)(cells + 1), st);
+  cub::DeviceRadixSort::SortPairs(tmp, sort_tmp, (const unsigned*)key, key2, (const int*)idx, idx2, (int)n, 0,
                                   bits, st);
   k_sap_gather<<<blocks(n, 256), 256, 0, st>>>(n, idx2, points01, normals, sp, sn);
   k_sap_splat<<<blocks(cells, 128), 128, 0, st>>>(res, start, sp, sn, grid);
@@ -401,7 +316,7 @@ int gsr_sap_spectral(int res, double sig, const float* spectrum, float* phi_hat,
 int gsr_sap_shift_scale(int64_t n, const float* points01, int res, const float* phi, gsr_alloc_fn scratch_alloc,
                         void* scratch_user, float* psi, void* stream) {
   const char* fn = "gsr_sap_shift_scale";
-  if (!n_ok(fn, n) || !res_ok(fn, res)) return -1;
+  if (!count_ok(fn, n, "n") || !res_ok(fn, res)) return -1;
   if (!points01 || !phi || !psi || !scratch_alloc) return fail(fn, "points01, phi, psi and scratch_alloc are required");
   cudaStream_t st = (cudaStream_t)stream;
   double* part = reinterpret_cast<double*>(scratch_alloc(scratch_user, (RED_CTAS + 1) * sizeof(double)));
@@ -421,36 +336,8 @@ int64_t gsr_sap_marching_cubes(int res, const float* psi, const float* transform
   if (!psi || !transform) return fail(fn, "psi and transform are required");
   if (!scratch_alloc || !vertex_alloc || !face_alloc || !n_faces)
     return fail(fn, "allocators and n_faces are required");
-  cudaStream_t st = (cudaStream_t)stream;
-  const long long N = (long long)res * res * res;
-  size_t scan_tmp = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (int*)nullptr, (int)(N + 1), st);
-  const size_t o_cube = 0, o_edges = align256(N), o_fb = o_edges + align256(N), o_vb = o_fb + align256((N + 1) * 4),
-               o_rb = o_vb + align256((N + 1) * 4), o_tmp = o_rb + 256, total = o_tmp + align256(scan_tmp);
-  char* s = scratch_alloc(scratch_user, total);
-  if (!s) return fail(fn, "scratch allocation failed");
-  unsigned char* cube = reinterpret_cast<unsigned char*>(s + o_cube);
-  unsigned char* edges = reinterpret_cast<unsigned char*>(s + o_edges);
-  int* fbase = reinterpret_cast<int*>(s + o_fb);
-  int* vbase = reinterpret_cast<int*>(s + o_vb);
-  long long* rb_dev = reinterpret_cast<long long*>(s + o_rb);
-  k_dmc_count<<<blocks(N + 1, 128), 128, 0, st>>>(res, psi, cube, edges, fbase, vbase);
-  cub::DeviceScan::ExclusiveSum(s + o_tmp, scan_tmp, fbase, (int)(N + 1), st);
-  cub::DeviceScan::ExclusiveSum(s + o_tmp, scan_tmp, vbase, (int)(N + 1), st);
-  k_dmc_counts<<<1, 1, 0, st>>>(vbase, fbase, N, rb_dev);
-  long long rb[2];
-  cudaMemcpyAsync(rb, rb_dev, sizeof(rb), cudaMemcpyDeviceToHost, st);
-  if (launched(fn)) return -1;
-  if (cudaStreamSynchronize(st) != cudaSuccess) { launched(fn); return -1; }
-  const long long V = rb[0], F = rb[1];
-  *n_faces = F;
-  if (V == 0 && F == 0) return 0;
-  char* verts = vertex_alloc(vertex_user, (size_t)V * 12);
-  char* faces = face_alloc(face_user, (size_t)F * 24);
-  if (!verts || !faces) return fail(fn, "output allocation failed");
-  k_dmc_emit<<<blocks(N, 128), 128, 0, st>>>(res, psi, cube, edges, vbase, fbase, transform,
-                                             reinterpret_cast<float*>(verts), reinterpret_cast<long long*>(faces));
-  return launched(fn) ? -1 : V;
+  return mc_dense<false>(fn, res, Outside{psi}, SapVertex{psi, transform}, scratch_alloc, scratch_user, vertex_alloc,
+                        vertex_user, face_alloc, face_user, n_faces, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -19,7 +19,6 @@ reference) is a uniform-grid search on the device as well (`knn`, gsr_knn_grid).
 Poisson solve + marching cubes) is CUDA kernels around torch's cuFFT (csrc/gsr_sap.cu, DESIGN.md 7h), and the
 point-cloud cleaning an exact k-nearest-neighbour search fused with its two consumers (csrc/gsr_clean.cu, DESIGN.md 7i).
 """
-import ctypes as C
 import math
 
 import numpy as np
@@ -228,7 +227,7 @@ def extract_pcd(renderer, pcd, cameras, d=3, sigma_color=75, sigma_space=75, smo
 
 
 # ---- Shape-as-Points meshing: the `--meshing sap` step of extract_pcd.py:397-399 (models/sap.py, DPSR) ----
-_SAP_SCRATCH, _SAP_VERTICES, _SAP_FACES = 1, 2, 3  # slots of _lib.scratch
+_SAP_SCRATCH = 1  # slot of _lib.scratch
 
 
 def _sap_inputs(points, normals, res, sig, what):
@@ -312,14 +311,7 @@ def mesh_sap(xyz, normals, res=256, sig=2):
     with _lib.scratch(dev):
         call("gsr_sap_normalize", dev, x.shape[0], ptr(x), ALLOC, _SAP_SCRATCH, ptr(points01), ptr(transform))
     psi = _sap_psi(points01, n, res, float(sig))
-    nf = C.c_int64(0)
-    with _lib.scratch(dev) as bufs:
-        nv = call("gsr_sap_marching_cubes", dev, res, ptr(psi), ptr(transform), ALLOC, _SAP_SCRATCH, ALLOC,
-                  _SAP_VERTICES, ALLOC, _SAP_FACES, C.byref(nf))
-    F = nf.value
-    v = bufs[_SAP_VERTICES].view(torch.float32).reshape(nv, 3) if nv else torch.empty(0, 3, device=dev)
-    f = bufs[_SAP_FACES].view(torch.int64).reshape(F, 3) if F else torch.empty(0, 3, dtype=torch.int64, device=dev)
-    return v, f
+    return _lib.call_mesh("gsr_sap_marching_cubes", dev, res, ptr(psi), ptr(transform))
 
 
 # ---- point-cloud cleaning: clean_point_cloud of extract_pcd.py:30-51 (csrc/gsr_clean.cu, DESIGN.md 7i) ----

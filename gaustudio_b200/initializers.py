@@ -308,7 +308,6 @@ def voxelize(vertices, faces, res, voxel_size):
 
 
 # ---- VisualHull (mask.py) and depth (depth.py): initializers that read posed views (csrc/gsr_hull.cu, DESIGN.md 7k) --
-_HULL_VERTICES, _HULL_FACES = 2, 3
 MAX_HULL_RES = 512  # the marching cubes' limit
 
 
@@ -397,14 +396,7 @@ def visual_hull_mesh(occ, threshold, radius, translate):
     if not 0.0 < threshold < 1.0:
         raise ValueError(f"threshold must be in (0, 1), got {threshold!r}")
     dev, occ = occ.device, occ.contiguous()
-    nf = C.c_int64(0)
-    with _lib.scratch(dev) as bufs:
-        nv = call("gsr_hull_marching_cubes", dev, res, ptr(occ), float(threshold), radius, *map(float, t), ALLOC,
-                  _SCRATCH, ALLOC, _HULL_VERTICES, ALLOC, _HULL_FACES, C.byref(nf))
-    F = nf.value
-    v = bufs[_HULL_VERTICES].view(torch.float32).reshape(nv, 3) if nv else torch.empty(0, 3, device=dev)
-    f = bufs[_HULL_FACES].view(torch.int64).reshape(F, 3) if F else torch.empty(0, 3, dtype=torch.int64, device=dev)
-    return v, f
+    return _lib.call_mesh("gsr_hull_marching_cubes", dev, res, ptr(occ), float(threshold), radius, *map(float, t))
 
 
 @register("VisualHull")

@@ -31,7 +31,7 @@ from . import _lib
 from ._lib import ALLOC, call, ptr
 from .extract import _extrinsics_host, _intrinsics_host, _need_cuda
 
-_SCRATCH, _VERTICES, _FACES = 1, 2, 3  # slots of _lib.scratch
+_SCRATCH = 1  # slot of _lib.scratch
 
 
 class TSDFVolume:
@@ -68,15 +68,7 @@ class TSDFVolume:
     def extract_triangle_mesh(self, min_weight=0.0):
         """-> (vertices [V,3] float32, faces [F,3] int64), CUDA.  Cubes of voxel centres whose 8 corners all have
         weight > min_weight; faces point towards positive tsdf (the observed side)."""
-        nf = C.c_int64(0)
-        with _lib.scratch(self.device) as bufs:
-            nv = call("gsr_tsdf_extract", self.device, ptr(self.state), self.capacity_bricks, float(min_weight), ALLOC,
-                      _SCRATCH, ALLOC, _VERTICES, ALLOC, _FACES, C.byref(nf))
-        F = nf.value
-        v = bufs[_VERTICES].view(torch.float32).reshape(nv, 3) if nv else torch.empty(0, 3, device=self.device)
-        f = bufs[_FACES].view(torch.int64).reshape(F, 3) if F else torch.empty(0, 3, dtype=torch.int64,
-                                                                             device=self.device)
-        return v, f
+        return _lib.call_mesh("gsr_tsdf_extract", self.device, ptr(self.state), self.capacity_bricks, float(min_weight))
 
     def export(self):
         """-> (brick_keys [n] int64, sums [n,512] int64, weights [n,512] int32) in key order: the raw volume state

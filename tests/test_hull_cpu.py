@@ -1,6 +1,7 @@
 """CPU: the VisualHull and depth initializers' restatements (tests/hull_ref64.py) against the reference's own outputs
 (tests/golden/hull_golden.npz, made by tests/golden/make_golden_hull.py), Camera's per-view fields and resizes, the
 hull mesh restatement's topology, and every refusal before any device call."""
+import math
 import os
 
 import numpy as np
@@ -9,7 +10,7 @@ import torch
 
 import hull_ref64 as R
 import sap_ref64
-from gaustudio_b200 import initializers
+from gaustudio_b200 import _lib, initializers
 from gaustudio_b200.camera import Camera, look_at_camera, orbit_cameras
 from gaustudio_b200.synthetic import GaussianPointCloud
 
@@ -208,3 +209,49 @@ def test_depth_refusals(tmp_path, no_device):
         init(model, cams)  # a CPU model, after the views passed
     assert cams[0].image_width == 40 and tuple(cams[0].depth.shape) == (32, 40)  # the caller's camera is untouched
     assert not os.path.exists(tmp_path / "fused.ply")
+
+
+# ---- refusals of the C entries: each check returns -1 with its text, before any device work ----
+_NULL_FN = _lib.ALLOC_FN()
+_FN = _lib.ALLOC_FN(lambda u, n: 0)
+_P = 1 << 20  # fake device address, never dereferenced: every call below is refused before any work
+RES = "res must be in 2..512"
+RADIUS = "radius must be positive and finite"
+TRANSLATE = "translate must be finite"
+C_CHECKS = [
+    ("gsr_hull_carve", dict(res=32, radius=1.0, tx=0.0, ty=0.0, tz=0.0, n_cams=2, proj=_P, views=_P, masks=_P,
+                            occ=_P, stream=None), [
+        (RES, [dict(res=1), dict(res=513), dict(res=-4)]),
+        (RADIUS, [dict(radius=0.0), dict(radius=-1.0), dict(radius=math.nan), dict(radius=math.inf),
+                  dict(radius=1e300)]),
+        (TRANSLATE, [dict(tx=math.nan), dict(ty=math.inf), dict(tz=-math.inf)]),
+        ("n_cams must be >= 0", [dict(n_cams=-1)]),
+        ("occ, proj and views are required", [dict(occ=None), dict(proj=None), dict(views=None)]),
+    ]),
+    ("gsr_hull_marching_cubes", dict(res=32, occ=_P, threshold=0.5, radius=1.0, tx=0.0, ty=0.0, tz=0.0,
+                                     scratch_alloc=_FN, scratch_user=None, vertex_alloc=_FN, vertex_user=None,
+                                     face_alloc=_FN, face_user=None, n_faces=_P, stream=None), [
+        (RES, [dict(res=1), dict(res=513)]),
+        ("threshold must be in (0, 1)", [dict(threshold=0.0), dict(threshold=1.0), dict(threshold=math.nan)]),
+        (RADIUS, [dict(radius=0.0), dict(radius=math.inf)]),
+        (TRANSLATE, [dict(tx=math.inf), dict(ty=math.nan), dict(tz=math.nan)]),
+        ("occ is required", [dict(occ=None)]),
+        ("allocators and n_faces are required",
+         [dict(scratch_alloc=_NULL_FN), dict(vertex_alloc=_NULL_FN), dict(face_alloc=_NULL_FN), dict(n_faces=None)]),
+    ]),
+]
+
+
+@pytest.mark.parametrize("entry,base,checks", C_CHECKS, ids=[c[0] for c in C_CHECKS])
+def test_c_refusals_fire_in_order_before_any_work(entry, base, checks):
+    """Each check returns -1 with its text, alone and together with the triggers of every later check."""
+    fn = getattr(_lib.lib(), entry)
+    for k, (err, variants) in enumerate(checks):
+        later = {}
+        for _, vs in reversed(checks[k + 1:]):
+            later.update(vs[0])
+        for v in variants:
+            for over in (v, {**later, **v}):
+                args = {**base, **over}
+                assert fn(*args.values()) == -1, (entry, over)
+                assert _lib.last_error() == f"{entry}: {err}", (entry, over, _lib.last_error())

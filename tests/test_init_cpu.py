@@ -7,7 +7,7 @@ import pytest
 import torch
 
 import init_ref64 as R
-from gaustudio_b200 import initializers
+from gaustudio_b200 import _lib, initializers
 from gaustudio_b200.synthetic import GaussianPointCloud
 
 
@@ -268,3 +268,81 @@ def test_initializer_refusals_before_device_work(tmp_path):
         initializers.dist2(torch.zeros(4, 3, dtype=torch.float64))
     with pytest.raises(ValueError):
         initializers.normal2rotation(torch.zeros(4, 2))
+
+
+# ---- refusals of the C entries: each check returns -1 with its text, before any device work ----
+_NULL_FN = _lib.ALLOC_FN()
+_FN = _lib.ALLOC_FN(lambda u, n: 0)
+_P = 1 << 20  # fake device address, never dereferenced: every call below is refused before any work
+
+
+def _range(what):
+    return f"{what} must be in 1..2^31-1"
+
+
+def _counts(*names):
+    return [dict({k: 0 for k in names}), dict({k: -1 for k in names}), dict({k: 1 << 31 for k in names})]
+
+
+VOX_RES = "res must be in 1..1024"
+C_CHECKS = [
+    ("gsr_dist2", dict(n=10, xyz=_P, scratch_alloc=_FN, scratch_user=None, dist2=_P, stream=None), [
+        (_range("n"), _counts("n")),
+        ("xyz, scratch_alloc and dist2 are required", [dict(xyz=None), dict(scratch_alloc=_NULL_FN), dict(dist2=None)]),
+    ]),
+    ("gsr_normal2rotation", dict(n=10, normals=_P, rot=_P, stream=None), [
+        (_range("n"), _counts("n")),
+        ("normals and rot are required", [dict(normals=None), dict(rot=None)]),
+        ("rot must be 16-byte aligned", [dict(rot=_P + 4), dict(rot=_P + 8)]),
+    ]),
+    ("gsr_mesh_vertex_normals", dict(nv=10, verts=_P, nf=4, faces=_P, scratch_alloc=_FN, scratch_user=None,
+                                     normals=_P, stream=None), [
+        (_range("nv"), _counts("nv")),
+        (_range("nf"), _counts("nf")),
+        ("nf must be below 2^31 / 3", [dict(nf=0x7fffffff // 3 + 1), dict(nf=0x7fffffff)]),
+        ("verts, faces, scratch_alloc and normals are required",
+         [dict(verts=None), dict(faces=None), dict(scratch_alloc=_NULL_FN), dict(normals=None)]),
+    ]),
+    ("gsr_mesh_gaussians", dict(nf=4, n=3, verts=_P, faces=_P, vertex_normals=_P, colors=None, xyz=_P, rot=_P,
+                                f_dc=_P, scale=_P, opacity=_P, stream=None), [
+        (_range("nf"), _counts("nf")),
+        ("n must be 1, 3, 4 or 6", [dict(n=0), dict(n=2), dict(n=5), dict(n=7), dict(n=-1)]),
+        ("verts, faces, vertex_normals and every output are required",
+         [dict(verts=None), dict(faces=None), dict(vertex_normals=None), dict(xyz=None), dict(rot=None),
+          dict(f_dc=None), dict(scale=None), dict(opacity=None)]),
+        ("rot must be 16-byte aligned", [dict(rot=_P + 4)]),
+    ]),
+    ("gsr_voxelize", dict(nv=10, verts=_P, nf=4, faces=_P, res=16, voxel_size=0.0625, alloc=_FN, column_user=None,
+                          hit_user=None, sort_user=None, out_user=None, n_pairs=_P, stream=None), [
+        (_range("nv"), _counts("nv")),
+        (_range("nf"), _counts("nf")),
+        (VOX_RES, [dict(res=0), dict(res=1025)]),
+        ("voxel_size must be positive and finite",
+         [dict(voxel_size=0.0), dict(voxel_size=-1.0), dict(voxel_size=math.nan), dict(voxel_size=math.inf)]),
+        ("verts, faces, alloc and n_pairs are required",
+         [dict(verts=None), dict(faces=None), dict(alloc=_NULL_FN), dict(n_pairs=None)]),
+    ]),
+    ("gsr_voxel_colors", dict(ncell=10, cells=_P, offsets=_P, tris=_P, res=16, voxel_size=0.0625, verts=_P, faces=_P,
+                              colors=_P, rgb=_P, stream=None), [
+        (_range("ncell"), _counts("ncell")),
+        (VOX_RES, [dict(res=0), dict(res=1025)]),
+        ("cells, offsets, tris, verts, faces, colors and rgb are required",
+         [dict(cells=None), dict(offsets=None), dict(tris=None), dict(verts=None), dict(faces=None),
+          dict(colors=None), dict(rgb=None)]),
+    ]),
+]
+
+
+@pytest.mark.parametrize("entry,base,checks", C_CHECKS, ids=[c[0] for c in C_CHECKS])
+def test_c_refusals_fire_in_order_before_any_work(entry, base, checks):
+    """Each check returns -1 with its text, alone and together with the triggers of every later check."""
+    fn = getattr(_lib.lib(), entry)
+    for k, (err, variants) in enumerate(checks):
+        later = {}
+        for _, vs in reversed(checks[k + 1:]):
+            later.update(vs[0])
+        for v in variants:
+            for over in (v, {**later, **v}):
+                args = {**base, **over}
+                assert fn(*args.values()) == -1, (entry, over)
+                assert _lib.last_error() == f"{entry}: {err}", (entry, over, _lib.last_error())
